@@ -10,8 +10,8 @@ import types
 REF_DIR = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")
 
 
-def available():
-    return os.path.isdir(os.path.join(REF_DIR, "pykg2vec"))
+def available(ref_dir=REF_DIR):
+    return os.path.isdir(os.path.join(ref_dir, "pykg2vec"))
 
 
 def install_stubs():
@@ -36,12 +36,13 @@ def install_stubs():
         sys.modules.update({"matplotlib": mpl, "matplotlib.pyplot": plt})
 
 
-def load():
-    """-> the imported `pykg2vec` package of baseline/_ref (raises ImportError when it is not installed)."""
-    if not available():
-        raise ImportError("baseline/_ref/pykg2vec not found — run baseline/install_ref.sh in the build container")
+def load(ref_dir=REF_DIR):
+    """-> the imported `pykg2vec` package installed in ref_dir (default baseline/_ref; raises ImportError when
+    it is not installed there)."""
+    if not available(ref_dir):
+        raise ImportError("%s/pykg2vec not found" % ref_dir)
     install_stubs()
-    if REF_DIR not in sys.path:
-        sys.path.insert(0, REF_DIR)
+    if ref_dir not in sys.path:
+        sys.path.insert(0, ref_dir)
     import pykg2vec
     return pykg2vec

@@ -2,6 +2,7 @@
 """bench.py — scored triples/sec (train + 1-vs-all eval), FB15k-237 shape, TransE d=200.
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA path
+    python bench.py --steps K --dump-outputs DIR             # + the outputs of the last timed step as DIR/*.npy
     python bench.py --impl reference --steps K --warmup W    # the UNMODIFIED reference on the host cores
 
 Workload (BASELINE.json configs[1]): TransE, N=14,541 entities, R=237 relations, d=200,
@@ -60,8 +61,8 @@ def peaks():
         with open(p) as f:
             d = json.load(f)
         return {"hbm": float(d["hbm_gbs"]), "bf16": float(d["bf16_tflops"]), "bf16_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
-                "src": "measured (MEASURED_PEAKS.json)", "sm_max": float(d.get("sm_max_mhz", 1965.0))}
-    return {"hbm": 6650.0, "bf16": 1590.0, "bf16_sustained": 1400.0, "src": "fallback (B200_PROFILING.md)", "sm_max": 1965.0}
+                "src": "measured (MEASURED_PEAKS.json)", "sm_max": float(d.get("sm_max_mhz", 1980.0))}
+    return {"hbm": 3350.0, "bf16": 989.0, "bf16_sustained": 989.0, "src": "NVIDIA H100 SXM data sheet (dense, 700 W)", "sm_max": 1980.0}
 
 
 class ClockSampler:
@@ -157,20 +158,9 @@ def event_ms(torch, fn, reps, flush=None):
     return tot / reps
 
 
-# DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of ONE `ncu --set full` capture of each
-# kernel at exactly the shapes timed here — the summaries are committed under profiles/ (ncu cannot run inside
-# this process, and a number printed under ncu is never a bench value).
-NCU_TRAFFIC = {
-    "tc_sweep_both": (13.101824e6 + 0.0, "profiles/r2_ncu_tc_sweep_final_summary.txt (cold caches: the 12 MB of bf16 "
-                                         "candidate operands read once from DRAM; in the step they are L2 hits)"),
-    "transe": (6.846856e9 + 19.496704e6, "profiles/r2_ncu_score_fwd_transe_staged_summary.txt"),
-    "complex": (6.801099e9 + 11.725824e6, "profiles/r2_ncu_score_fwd_complex_summary.txt"),
-}
-
-
 def gather_score_rooflines(torch, _lib, dev, pk, reps=10):
     """The fused gather+score kernels north_star's >= 60 %-of-HBM target names (TransE, ComplEx; d = 200),
-    timed here on tables far larger than the 126 MB L2 with random ids.  Algorithmic bytes count what
+    timed here on tables far larger than the 50 MB L2 with random ids.  Algorithmic bytes count what
     must come from DRAM: the ENTITY rows (2 per triple for TransE, 4 for ComplEx), the 24 B of ids and the
     4 B score — the R=1000 relation rows are L2 hits and are not counted."""
     out = []
@@ -194,8 +184,7 @@ def gather_score_rooflines(torch, _lib, dev, pk, reps=10):
                     "frac": alg / (ms * 1e-3) / 1e9 / pk["hbm"], "peak_source": pk["src"], "launch_ms": ms,
                     "algorithmic_bytes_per_launch": alg,
                     "algorithmic_bytes_per_triple": "entity rows %d x %d B + 24 B ids + 4 B score (relation rows are L2-resident)"
-                                                    % (2 * ntab_e, d * 4),
-                    "traffic": NCU_TRAFFIC[name][0], "traffic_source": NCU_TRAFFIC[name][1]})
+                                                    % (2 * ntab_e, d * 4)})
         del tabs, desc, h, r, t, o
         torch.cuda.empty_cache()
     return out
@@ -242,13 +231,15 @@ def run_cuda(args):
     def train_resident(i):
         tr.train_batch_device(devin[i][0])   # fused step; at world > 1 data-parallel inside the Trainer
 
+    last = {}   # device tensors the last resident step returned to its caller (--dump-outputs)
+
     def resident_step(i):
         if graph_step is not None:
             return graph_step(i)
         # multi-GPU "ids" mode: the 24 KB id all-gather is started first and hides behind the evaluation batch
         ex = tr.exchange_batch_async(devin[i][0])
         eval_resident(i)
-        tr.train_batch_device(devin[i][0], exchanged=ex)
+        last["loss"] = tr.train_batch_device(devin[i][0], exchanged=ex)
 
     # Single GPU: the resident step is ~12 short kernels, so launch gaps are a visible share of it.  It is
     # captured ONCE as a CUDA graph reading from fixed device buffers; a timed step is then the D2D copies of
@@ -313,6 +304,7 @@ def run_cuda(args):
                 _lib.train_pairwise_hinge_sgd(desc, scratch, *s_ids, w["margin"], lr, loss_buf)
 
             g, kernels_per_replay = capture(lambda: body(w["lr"]), lambda: body(0.0))
+            last["loss"] = loss_buf
             # the two halves as graphs of their own, for the separately reported train / eval rates
             g_eval, _ = capture(body_eval, body_eval)
             g_train, _ = capture(lambda: _lib.train_pairwise_hinge_sgd(desc, scratch, *s_ids, w["margin"], w["lr"], loss_buf),
@@ -341,7 +333,7 @@ def run_cuda(args):
                 return [gl[k] for k in range(6)]
 
             def body_train():
-                tr.train_batch_device(s_ids, exchanged=glob_ids)
+                last["loss"] = tr.train_batch_device(s_ids, exchanged=glob_ids)
 
             def warm_train():
                 lr0 = tr.config.learning_rate
@@ -442,7 +434,10 @@ def run_cuda(args):
 
     # sustained run (~1.5 s of back-to-back steps) so that nvidia-smi samples clocks UNDER LOAD.  The number of
     # passes is fixed from one timed pass and agreed across ranks (MAX): a time-based loop would let the ranks
-    # run different numbers of steps, and the steps contain collectives.
+    # run different numbers of steps, and the steps contain collectives.  Its training updates are rolled back
+    # afterwards, so that the timed steps start from the same tables on every run of the same arguments.
+    tables = [t_.detach() for t_ in tr.model.kge_tables()]
+    saved_tables = [t_.clone() for t_ in tables]
     torch.cuda.synchronize()
     t_p0 = time.perf_counter()
     for i in range(args.warmup, total):
@@ -460,6 +455,9 @@ def run_cuda(args):
             resident_step(i)
         torch.cuda.synchronize()
     ms_sustained = (time.perf_counter() - t_s0) * 1e3 / (n_pass * args.steps)
+    for t_, s_ in zip(tables, saved_tables):
+        t_.copy_(s_)
+    del saved_tables
     barrier()
     import gc
     gc.collect()
@@ -467,11 +465,15 @@ def run_cuda(args):
     launches0 = _lib.launch_count()
     ms_res = max_over_ranks(timed(resident_step, args.warmup, args.steps, True))
     launches = _lib.launch_count() - launches0
+    if args.dump_outputs and rank == 0:
+        dumped = {"rank_counts": counts.double(), "loss": last["loss"].float().reshape(-1)}
+        dumped.update(("table%d" % k, t_.float()) for k, t_ in enumerate(tables))
+        dumped = {k: v.cpu().numpy() for k, v in dumped.items()}   # (copies: later legs keep updating the tables)
     if graph_step is not None:
         launches = kernels_per_replay * args.steps   # replays re-execute the captured kernels
     ms_train = max_over_ranks(timed(train_resident, args.warmup, args.steps, True))
     ms_eval = max_over_ranks(timed(eval_resident, args.warmup, args.steps, True))
-    # warm-L2 back-to-back variant (tables stay in the 126 MB L2 between steps, as in a real epoch)
+    # warm-L2 back-to-back variant (tables stay in the 50 MB L2 between steps, as in a real epoch)
     barrier()
     a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     a.record()
@@ -539,7 +541,7 @@ def run_cuda(args):
         "gpu_launches": int(launches),
         "clocks": clocks,
         "roofline": {"kernel": "tc_sweep_kernel: 1-vs-all tensor-core sweep (%s, Q=512 x N=14541 x d=200 each, "
-                               "tcgen05.mma bf16x3 split, fp32 accumulation in TMEM)"
+                               "wgmma bf16x3 split, fp32 accumulation in registers)"
                                % ("tail + head directions in one launch" if tc_dirs == 2 else "tail direction"),
                      "directions_per_launch": tc_dirs,
                      "bound": "tensor", "achieved": alg_flops / (tc_ms * 1e-3) / 1e12, "peak": pk["bf16"], "unit": "TFLOP/s",
@@ -548,15 +550,23 @@ def run_cuda(args):
                      "algorithmic_flops_per_unit": "2*d = 400 flop per scored candidate (one length-d contraction)",
                      "executed_tensor_flops_per_launch": exec_flops,
                      "executed_frac": exec_flops / (tc_ms * 1e-3) / 1e12 / pk["bf16"],
-                     "traffic": NCU_TRAFFIC["tc_sweep_both"][0] if tc_dirs == 2 else None,
-                     "traffic_source": NCU_TRAFFIC["tc_sweep_both"][1] if tc_dirs == 2 else None,
                      "note": "exact fp32 ranks need three bf16 passes (a0b0 + a0b1 + a1b0) over tiles padded to 128 x 128 x 208: "
                              "executed_frac counts those tensor flops, frac only the algorithm's 2*Q*N*d",
                      "fp32_sweep_ms_per_direction": fp32_ms, "speedup_vs_fp32_sweep": fp32_ms * tc_dirs / tc_ms},
         "rooflines_extra": extra,
         "cpu_baseline": cpu,
     }
+    if args.dump_outputs:
+        write_outputs(args.dump_outputs, dumped)
     return line
+
+
+def write_outputs(dirpath, arrays):
+    """DIR/<name>.npy for every output array (float32 / float64 as given)."""
+    os.makedirs(dirpath, exist_ok=True)
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    for name, a in arrays.items():
+        np.save(os.path.join(dirpath, name + ".npy"), a)
 
 
 # ------------------------------------------------------------------ CPU reference arm ----
@@ -776,6 +786,9 @@ def main():
                          "across the ranks) — bench_sharded.py, one JSON line each, not the driver's contract line")
     ap.add_argument("--no-graph", action="store_true",
                     help="launch the resident step kernel by kernel instead of replaying it as one CUDA graph (N = 1)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (rank counts [Q,4] as float64, "
+                         "the training loss, the updated embedding tables as float32) to DIR/<name>.npy")
     ap.add_argument("--lite", action="store_true",
                     help="profiling aid: only the HBM-resident leg (no e2e / CPU baseline / self-check); never a bench value")
     args = ap.parse_args()

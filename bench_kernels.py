@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Per-kernel roofline sweep (NOT the driver's bench.py): fused gather+score forward /
-backward / fused train step on tables far larger than the 126 MB L2, random ids, so the row
+backward / fused train step on tables far larger than the 50 MB L2, random ids, so the row
 gathers really come from HBM.  Prints one JSON line per case:
 
     achieved GB/s = ALGORITHMIC bytes (SURVEY.md 8d: rows*d*4 + 24 B ids + 4 B score per triple;

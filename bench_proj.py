@@ -4,7 +4,7 @@ shape (N=14,541, R=237, hidden_size 200 as a 20x20 image), training batch B=128 
 batch Q=512, CUDA events, L2 flushed between repetitions.  One JSON line per measurement:
 
   flops  = algorithmic fp32 FLOPs of the op (2*M*N*K per GEMM use)
-  frac   = flops / time / fp32 FMA-pipe peak (148 SMs x 128 lanes x 2 x SM clock) — the tiled GEMM is
+  frac   = flops / time / fp32 FMA-pipe peak (132 SMs x 128 lanes x 2 x SM clock, H100 SXM) — the tiled GEMM is
            bound by the fp32 pipe, not HBM (its operands are re-used on chip; ranks must be exact in
            fp32, so no tensor-core formulation in this round)
   bytes  = algorithmic HBM bytes (operands once + outputs once), GBps = bytes / time
@@ -26,7 +26,7 @@ sys.path.insert(0, ROOT)
 from pykg2vec_b200 import _lib, import_model  # noqa: E402
 
 N, R, K, K1 = 14541, 237, 200, 20
-SM, LANES, CLOCK_GHZ = 148, 128, 1.965
+SM, LANES, CLOCK_GHZ = 132, 128, 1.98
 FP32_PEAK_TFLOPS = SM * LANES * 2 * CLOCK_GHZ / 1e3
 
 
@@ -36,7 +36,7 @@ def time_ms(fn, reps, flush):
     torch.cuda.synchronize()
     total = 0.0
     for _ in range(reps):
-        flush.zero_()                    # 256 MiB > the 126 MB L2
+        flush.zero_()                    # 256 MiB > the 50 MB L2
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record()
         fn()

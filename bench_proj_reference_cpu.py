@@ -1,14 +1,14 @@
 #!/usr/bin/env python
 """CPU timing of the UNMODIFIED reference ConvE (pykg2vec/models/projection.py:12-125) on the workload
-bench_proj.py times on the B200: FB15k-237 shape (N=14,541, R=237, hidden_size 200 as 20x20),
+bench_proj.py times on the GPU: FB15k-237 shape (N=14,541, R=237, hidden_size 200 as 20x20),
   * evaluation as the reference runs it (evaluator.py:309-334): per test triple one predict_tail_rank and
     one predict_head_rank — a [1,N] forward + topk(N) each — and the Python rank walk of MetricCalculator;
   * one training step (trainer.py:159-174,298-299): both directions, multi_class_bce with label smoothing,
     backward, adam, batch 128, dense [128,N] label matrices.
-Needs /root/reference, so it runs in the BUILD CONTAINER only (its host cores, stated in the output), not
-on the GPU box: the numbers are an indication beside profiles/r1_proj_kernels_v2.jsonl, not a bench value.
+Needs the reference package installed (baseline/install_ref.sh) and runs on host cores (stated in the output):
+the numbers are an indication beside bench_proj.py's, not a bench value.
 
-    python bench_proj_reference_cpu.py [--queries 40] [--steps 5] [--out profiles/r1_conve_cpu_reference_v1.json]
+    python bench_proj_reference_cpu.py [--queries 40] [--steps 5] [--out FILE.json]
 """
 import argparse
 import json

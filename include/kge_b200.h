@@ -1,5 +1,5 @@
 /*
- * kge_b200.h — C-ABI of the B200-native KGE scoring engine (libkge_b200.so).
+ * kge_b200.h — C-ABI of the H100-native (sm_90a) KGE scoring engine (libkge_b200.so).
  *
  * The reference (Sujit-O/pykg2vec) has NO native interface: its hot path is the
  * duck-typed Python surface `model.forward(h, r, t)` / `model.loss(...)` /
@@ -262,8 +262,8 @@ int kge_rank_last_sweep_directions(void);
 int kge_debug_set_tc_trace(long long* buf);
 
 /* Two-level exact sweep (TransE -l1 False, DistMult, CP, ComplEx, RESCAL, RotatE; >= 1024 candidate rows):
- * level 1 evaluates the Q x N x K contraction on the tensor cores (tcgen05.mma, bf16 x 3 split, fp32
- * accumulation in TMEM) and counts every candidate whose accumulator clears the query's threshold by
+ * level 1 evaluates the Q x N x K contraction on the tensor cores (wgmma, bf16 x 3 split, fp32
+ * accumulation in registers) and counts every candidate whose accumulator clears the query's threshold by
  * more than a proven error bound of that (query, candidate) pair; level 2 re-evaluates the few (query, candidate) pairs inside the
  * band in the canonical fp32 arithmetic.  The counts equal the fp32 specification's for every input
  * (DESIGN.md §4b).  kge_rank_tc_probe exposes level 1 of ONE direction (0 tail, 1 head) for tests and
@@ -296,7 +296,7 @@ int kge_project_entities(const kge_model_t* m, int64_t r, float* out, void* stre
  * the canonical arithmetic: row * (1 / max(|row|, 1e-12))), TransE of width rel_dim over
  * [out, normalised rel] applies the reference's second normalisation (:463-465) and reproduces
  * score_TransR bit for bit.  (Proved on the oracle with the emulated kernels, tests/test_emu_project.py;
- * the relation-grouped Evaluator uses it for TransR only on request — not yet timed on a B200.) */
+ * the relation-grouped Evaluator uses it for TransR only on request — not timed.) */
 int kge_normalize_rows_to(const float* table, int64_t rows, int64_t width, float* out, void* stream);
 
 /* ---- projection-model tail: x.E^T + b -> sigmoid, multi-class BCE, rank counts ----------

@@ -1,6 +1,6 @@
 """Workload for compute-sanitizer (memcheck / racecheck / synccheck): every kernel with hand-rolled
-cross-warp synchronisation or atomics, at small sizes — the tensor-core sweep (TMA + mbarrier + tcgen05 +
-TMEM), the fp32 tiled sweep (TMA + mbarrier + release counters; whole-row and slab mode, all OPs), the
+cross-warp synchronisation or atomics, at small sizes — the tensor-core sweep (TMA + mbarrier +
+wgmma), the fp32 tiled sweep (TMA + mbarrier + release counters; whole-row and slab mode, all OPs), the
 exact-resolve kernel, the fp32 sweep's commit-or-fallback entry, the fused hinge step (atom.exch sparse apply), the
 fused RotatE self-adversarial step (warp team and CTA team) and the dense optimizer.  Results are checked against the oracle so a silent corruption would also fail here.
 

@@ -40,7 +40,8 @@ for mode in (os.environ.get("TC_TRACE_MODES", "0").split(",")):
     spans = spans[spans[:, 0] != 0]
     t0 = t[2, 63]
     out = {"directions": _lib.rank_last_sweep_directions(), "epi_mode": mode, "kernel_ms_untraced": times, "kernel_ms_traced": ms}
-    for r, name in enumerate(("producer", "mma", "epilogue")):
+    # role 0: the TMA producer's stage waits; 1: consumer warpgroup start (warp 4); 2: epilogue begin / end per tile
+    for r, name in enumerate(("producer", "consumer_start", "epilogue")):
         out[name] = [int(x - t0) for x in t[r, :62] if x != 0]
     if len(spans):
         s0 = spans[:, 0].min()

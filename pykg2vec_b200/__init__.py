@@ -1,4 +1,4 @@
-"""pykg2vec_b200 — B200-native (sm_100a) scoring engine behind pykg2vec's model surface.
+"""pykg2vec_b200 — H100-native (sm_90a) scoring engine behind pykg2vec's model surface.
 
 Package layout (only what the hot path needs):
   csrc/        CUDA kernels + the C-ABI (include/kge_b200.h)  -> _build/libkge_b200.so

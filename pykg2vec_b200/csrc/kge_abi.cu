@@ -29,8 +29,8 @@ int sm_count() {
   static thread_local int cached = 0;
   if (cached) return cached;
   int dev = 0, n = 0;
-  if (cudaGetDevice(&dev) != cudaSuccess) return 148;
-  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 148;
+  if (cudaGetDevice(&dev) != cudaSuccess) return 132;
+  if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) return 132;
   cached = n;
   return n;
 }
@@ -54,7 +54,7 @@ int num_tables(int model) {
 extern "C" {
 
 int kge_abi_version(void) { return KGE_ABI_VERSION; }
-const char* kge_version(void) { return "kge_b200 0.1 (sm_100a)"; }
+const char* kge_version(void) { return "kge_b200 0.1 (sm_90a)"; }
 const char* kge_last_error(void) { return kge::g_err; }
 int64_t kge_launch_count(void) { return (int64_t)kge::g_launches.load(std::memory_order_relaxed); }
 

@@ -1,4 +1,4 @@
-// kge_common.cuh — shared device/host helpers of libkge_b200.so (sm_100a only).
+// kge_common.cuh — shared device/host helpers of libkge_b200.so (sm_90a only).
 //
 // Canonical arithmetic (DESIGN.md §3): every score is evaluated with explicitly
 // rounded fp32 intrinsics (__fmaf_rn/__fadd_rn/__fmul_rn: never contracted or

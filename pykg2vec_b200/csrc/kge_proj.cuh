@@ -316,10 +316,7 @@ enum { PROJ_TILE_64x64 = 0, PROJ_TILE_64x128 = 1, PROJ_TILE_128x128 = 2 };
 inline int proj_tile_rows(int tile) { return tile == PROJ_TILE_128x128 ? 128 : 64; }
 inline int proj_tile_cols(int tile) { return tile == PROJ_TILE_64x64 ? 64 : 128; }
 // Large tiles halve the shared-memory operand traffic per fma (a 16-byte read feeds 32 fma instead
-// of 16) but need enough CTAs to fill 148 SMs.  Measured on the FB15k-237 ConvE shape
-// (profiles/r1_proj_kernels_v2.jsonl): Q=512 -> 128x128 is the fastest counting launch (0.140 vs
-// 0.156 ms for 64x64), B=128 -> 64x128 (0.040 vs 0.043 ms); the forward store launch is within 5 %
-// for all three.
+// of 16) but need enough CTAs to fill every SM: the largest tile that still gives two CTAs per SM.
 inline int proj_pick_tile(long long M, long long N, int sms) {
   if (((M + 127) / 128) * ((N + 127) / 128) >= 2ll * sms) return PROJ_TILE_128x128;
   if (((M + 63) / 64) * ((N + 127) / 128) >= (long long)sms) return PROJ_TILE_64x128;

@@ -1,4 +1,4 @@
-// kge_rank_tc.cu — 1-vs-all sweep on the 5th-generation tensor cores (tcgen05 + TMEM), EXACT.
+// kge_rank_tc.cu — 1-vs-all sweep on the Hopper tensor cores (wgmma + TMA + mbarrier), EXACT.
 //
 // The batched 1-vs-all sweep of the dot-product / squared-distance models (DistMult, CP, ComplEx,
 // RESCAL's h^T M_r . t, TransE-L2, RotatE) is a Q x N x K contraction.  Ranks, however, are
@@ -7,9 +7,9 @@
 //
 //   level 1 (this file, tensor cores): every fp32 operand x is split into two bf16 terms
 //       x0 = bf16_rn(x), x1 = bf16_rn(x - x0)            (|x - x0 - x1| <= 2^-18 |x|)
-//     and D(q,c) = sum_k a0 b0 + a0 b1 + a1 b0 is accumulated in fp32 in TMEM by three
-//     tcgen05.mma (kind::f16, bf16 inputs) passes per 16-wide k-step; operand tiles arrive by TMA
-//     (128-byte swizzle), accumulators are double buffered in TMEM and read back by tcgen05.ld.
+//     and D(q,c) = sum_k a0 b0 + a0 b1 + a1 b0 is accumulated in fp32 registers by three
+//     wgmma.mma_async (m64n128k16, bf16 inputs) per 16-wide k-step and warpgroup; operand tiles arrive
+//     by TMA (128-byte swizzle) through a ring of shared-memory stages guarded by mbarriers.
 //     Squared distances use |q - c|^2 = |q|^2 - 2 (q.c - |c|^2/2): the candidate norm term rides
 //     in three extra k-columns (a 3-way bf16 split of |c|^2/2 against -1), so the epilogue only
 //     compares the accumulator with two per-query constants:
@@ -41,12 +41,11 @@
 
 namespace kge {
 
-constexpr int kTcBM = 128;        // queries per CTA (UMMA M)
-constexpr int kTcBN = 128;        // candidates per tile (UMMA N)
-constexpr int kTcBKMax = 64;      // bf16 elements per k-block: 64 (128-byte swizzle rows) or 32 (64-byte rows; twice the stages)
-constexpr int kTcThreads = 320;   // warp 0: TMA producer, warp 1: MMA issuer + TMEM owner, warps 2-9: epilogue
-constexpr int kTcEpiWarps = 8;    // two warps per TMEM lane quadrant, each scanning half of the tile's columns
-constexpr int kTcTmemCols = 256;  // two accumulator stages of kTcBN fp32 columns (+ 256 for the query operands in a_tmem mode)
+constexpr int kTcBM = 128;        // queries per CTA: two consumer warpgroups of 64 rows (wgmma M = 64)
+constexpr int kTcBN = 128;        // candidates per tile (wgmma N)
+constexpr int kTcBK = 64;         // bf16 elements per k-block: one 128-byte swizzle row
+constexpr int kTcThreads = 384;   // warpgroup 0: TMA producer (one thread), warpgroups 1-2: wgmma + epilogue
+constexpr int kTcConsumerWarps = 8;
 constexpr int kTcMaxStages = 8;
 constexpr int kTcResidentMaxK = 256;                   // query block stays in smem when Kp <= 256
 
@@ -58,7 +57,6 @@ struct TcDirView {
   int32_t* tc_counts;      // [Q]
   unsigned* ctrl;          // [0] list length, [1] overflow ([2], [3] unused)
   unsigned long long* list;
-  const __nv_bfloat16* A0; const __nv_bfloat16* A1;   // [Q][Kp] query operands (read by the TMEM fill)
   float* dbg;              // optional [Q][nc] raw accumulators (tests)
 };
 struct TcParams {
@@ -67,19 +65,13 @@ struct TcParams {
   unsigned cap;
   int64_t Q, nc;
   int Kp, nkb, a_resident, nstages;
-  int bk;                  // k-block width in bf16 elements (64 or 32)
-  int a_tmem;              // the query block's operands live in TENSOR MEMORY (Kp <= 256): only the candidate tiles use smem
-  uint32_t tile_bytes;     // one operand k-block tile: 128 rows x bk x 2 bytes
+  uint32_t tile_bytes;     // one operand k-block tile: 128 rows x kTcBK x 2 bytes
   int tiles_per_cta, ntiles;
   long long* trace;        // optional timeline of CTA (0,0): [3 roles][64] clock64 stamps (kge_debug_set_tc_trace)
-  int epi_mode;            // measurement aid (KGE_TC_EPI_MODE): 0 normal, 1 load only, 2 count only (no band listing)
-  // exact-width last k-block: when Kp leaves 16 or 32 columns for it, it is staged as a narrow tile
-  // (32- / 64-byte rows, matching swizzle) instead of a zero-filled 128-byte one; 0 = treat it like the others
-  int tail_cols;
-  uint32_t tail_bytes;     // bytes of one operand's tail tile (128 rows x tail_cols x 2)
+  int epi_mode;            // measurement aid (KGE_TC_EPI_MODE): 0 normal, 1 MMA only, 2 count only (no band listing)
 };
-// a*: query operands of blockIdx.z == 0, c*: of blockIdx.z == 1; *t: the narrow tail k-block; in PAIR mode the b* boxes hold 64 rows
-struct TcMaps { CUtensorMap a0, a1, b0, b1, a0t, a1t, b0t, b1t, c0, c1, c0t, c1t; };
+// a*: query operands of blockIdx.z == 0, c*: of blockIdx.z == 1, b*: candidate operands
+struct TcMaps { CUtensorMap a0, a1, b0, b1, c0, c1; };
 
 // ---- PTX wrappers ---------------------------------------------------------------------------------
 KGE_DEV uint32_t tc_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -104,7 +96,7 @@ KGE_DEV void tc_mbar_wait(uint64_t* bar, uint32_t parity) {
         "selp.u32 %0, 1, 0, p;\n\t}"
         : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
     if (ok) return;
-    if (clock64() - t0 > 4000000000LL) __trap();   // ~2 s at 1.9 GHz
+    if (clock64() - t0 > 4000000000LL) __trap();   // ~2 s at 1.98 GHz
   }
 }
 KGE_DEV void tc_tma_load_2d(uint32_t dst_smem, const CUtensorMap* tm, int col, int row, uint64_t* bar) {
@@ -113,91 +105,47 @@ KGE_DEV void tc_tma_load_2d(uint32_t dst_smem, const CUtensorMap* tm, int col, i
       ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(tm)), "r"(col), "r"(row), "r"(tc_smem_u32(bar))
       : "memory");
 }
-// the same tile delivered to the CTAs named by `mask` of this cluster (same CTA-relative smem offset and
-// mbarrier in each): one L2 read, one TMA row request, several destinations
-KGE_DEV void tc_tma_load_2d_mc(uint32_t dst_smem, const CUtensorMap* tm, int col, int row, uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%2, %3}], [%4], %5;"
-      ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(tm)), "r"(col), "r"(row), "r"(tc_smem_u32(bar)), "h"(mask)
-      : "memory");
-}
-KGE_DEV void tc_cluster_sync() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-KGE_DEV void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-KGE_DEV void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// arrives on the mbarrier at `bar`'s offset in EVERY CTA of `mask` when the MMAs issued so far have completed
-KGE_DEV void tc_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(tc_smem_u32(bar)), "h"(mask) : "memory");
-}
-KGE_DEV void tc_commit(uint64_t* bar) {   // arrives on `bar` when every MMA issued so far by this thread has completed
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];"
-               ::"r"(tc_smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] . B[smem]^T, bf16 inputs, fp32 accumulate, M = 128, N = kTcBN, K = 16
-KGE_DEV void tc_mma(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// same with the A operand read from tensor memory (row i in lane i, two bf16 per 32-bit column): the
-// shared-memory traffic of an MMA halves (only B), which is what bounded the all-smem form at N = 128
-KGE_DEV void tc_mma_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-KGE_DEV void tc_tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};"
-               ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]) : "memory");
-}
-KGE_DEV void tc_tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 
-// shared-memory matrix descriptor: K-major operand tile [rows][64 bf16] written by TMA with the
-// 128-byte swizzle.  start address >> 4 in bits [0,14); leading byte offset (unused for swizzled
-// K-major, canonical value 1) in [16,30); stride byte offset = 8 rows x 128 B = 1024 (>> 4) in
-// [32,46); descriptor version 1 in [46,48); layout type SWIZZLE_128B = 2 in [61,64).
-// row_bytes = 128 (SWIZZLE_128B, layout 2), 64 (SWIZZLE_64B, 4) or 32 (SWIZZLE_32B, 6); the stride between
-// 8-row groups is 8 * row_bytes.
-KGE_DEV uint64_t tc_smem_desc(uint32_t addr, uint32_t row_bytes = 128u) {
-  const uint64_t layout = row_bytes == 128u ? 2u : (row_bytes == 64u ? 4u : 6u);
+// shared-memory matrix descriptor (sm_90 wgmma): K-major operand tile [rows][64 bf16] written by TMA with the
+// 128-byte swizzle.  start address >> 4 in bits [0,14); leading byte offset (unused for swizzled K-major,
+// canonical value 1) in [16,30); stride byte offset = 8 rows x 128 B = 1024 (>> 4) in [32,46); layout type
+// SWIZZLE_128B = 1 in [62,64).  16 bf16 further along k = 32 bytes further along the swizzled row: +2.
+KGE_DEV uint64_t tc_smem_desc(uint32_t addr) {
   uint64_t d = 0;
   d |= (uint64_t)((addr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;
-  d |= (uint64_t)((8u * row_bytes) >> 4) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= layout << 61;
+  d |= (uint64_t)(1024u >> 4) << 32;
+  d |= (uint64_t)1 << 62;
   return d;
 }
-// instruction descriptor (kind::f16): D fp32 (bits [4,6) = 1), A and B bf16 ([7,10) = [10,13) = 1),
-// both K-major (bits 15, 16 = 0), N >> 3 in [17,23), M >> 4 in [24,29)
-constexpr uint32_t kTcIdesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kTcBN >> 3) << 17) |
-                              ((uint32_t)(kTcBM >> 4) << 24);
+KGE_DEV void tc_wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+KGE_DEV void tc_wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+KGE_DEV void tc_wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-KGE_DEV void tc_tmem_ld32(uint32_t taddr, uint32_t (&v)[32]) {
+// d[64] (+)= A[smem, 64 x 16] . B[smem, 128 x 16]^T, bf16 inputs, fp32 accumulate, both operands K-major.
+// Fragment of thread (warp w of the warpgroup, lane l): d[4j + 2i + c] = row 16w + l/4 + 8i, column 8j + 2(l%4) + c.
+KGE_DEV void tc_wgmma(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
       "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr) : "memory");
+      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+      "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+      "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(adesc), "l"(bdesc), "r"(accumulate)
+      : "memory");
 }
-KGE_DEV uint32_t tc_tmem_ld1(uint32_t taddr) {
-  uint32_t v;
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x1.b32 {%0}, [%1];" : "=r"(v) : "r"(taddr) : "memory");
-  return v;
-}
-KGE_DEV void tc_tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
 // timeline stamps of CTA (0,0) (measurement aid; P.trace is null in normal operation)
 #define TC_STAMP(role, slot)                                                                         \
@@ -205,10 +153,10 @@ KGE_DEV void tc_tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" :
     if (P.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (slot) < 64 && ((slot) < 62 || (slot) == 63)) P.trace[(role) * 64 + (slot)] = clock64(); \
   } while (0)
 
-// Pair-list slots are handed out per WARP in blocks (16 slots) reserved with one global atomic (a returning atomic
-// per ambiguous pair stalled the whole epilogue: 8k of 10k cycles per tile, profiles/r2_tc_trace_v2_*):
-// base/size = the warp's current block in P.list, used = slots already written.  Unused slots of a block
-// are filled with the sentinel ~0 (band_resolve_kernel skips them), so [0, ctrl[0]) is always fully defined.
+// Pair-list slots are handed out per WARP in blocks (16 slots) reserved with one global atomic (a returning
+// atomic per ambiguous pair would stall the epilogue on its round trip): base/size = the warp's current block
+// in P.list, used = slots already written.  Unused slots of a block are filled with the sentinel ~0
+// (band_resolve_kernel skips them), so [0, ctrl[0]) is always fully defined.
 struct TcListState { unsigned base, used, size; };
 constexpr unsigned long long kTcListHole = ~0ull;
 constexpr unsigned kTcListBlock = 16;
@@ -230,67 +178,37 @@ KGE_DEV void tc_list_pad(TcListState& L, const TcParams& P, const TcDirView& V, 
   L.used = L.size;
 }
 
-// 32 accumulator columns (= candidates cbase .. cbase+31) of this thread's query row: count the
-// certainly-better ones.  Per column: the band half-width of the pair (two fma on the candidate's norm
-// bound, broadcast from the lane that loaded it), u = D - centre, 2 compares + 2 predicated adds, two
-// independent chains; warps in which some row has candidates inside its band list them from the registers
-// already loaded — a warp-level exclusive scan assigns the slots, no atomic on the path.
+// The band test of one accumulator: half-width of the pair from the candidate's norm bound (two fma),
+// u = D - centre; certainly better when u > half, inside the band when -half <= u <= half.
 struct TcBand { float centre, a, b, e; };
 KGE_DEV void tc_band_eval(const TcBand& Bq, float x, float n, float& u, float& half) {
   half = __fmaf_rn(__fmaf_rn(Bq.e, n, Bq.b), n, Bq.a);
   u = __fsub_rn(x, Bq.centre);
 }
-KGE_DEV int tc_scan_chunk(const uint32_t (&v)[32], int nv, const TcBand& Bq, float nl, int64_t q, int64_t cbase,
-                          bool live, const TcParams& P, const TcDirView& V, TcListState& L, int lane, int& ev, bool stamp) {
-  if (P.epi_mode == 1) return (int)(v[0] & 1u) + (int)(v[31] & 1u);
-  if (stamp) TC_STAMP(2, ev++);
-  int hi0 = 0, hi1 = 0, lo0 = 0, lo1 = 0;
-#define TC_CMP(HI, LO, X, J)                                                                              \
-  do {                                                                                                    \
-    float u_, h_;                                                                                         \
-    tc_band_eval(Bq, X, __shfl_sync(0xffffffffu, nl, J), u_, h_);                                         \
-    asm("{\n\t.reg .pred p, q;\n\t.reg .f32 nh;\n\tneg.f32 nh, %3;\n\tsetp.gt.f32 p, %2, %3;\n\t"       \
-        "setp.ge.f32 q, %2, nh;\n\t@p add.s32 %0, %0, 1;\n\t@q add.s32 %1, %1, 1;\n\t}"                  \
-        : "+r"(HI), "+r"(LO) : "f"(u_), "f"(h_));                                                         \
-  } while (0)
-  if (nv == 32) {
+
+// Epilogue of one 64 x 128 accumulator tile held by a warpgroup: this thread's rows qa (= q of i = 0) and qa + 8,
+// columns 8j + 2(lane%4) + c of the tile (cbase + ...).  Counts the certainly-better candidates per row; warps in
+// which some pair lies inside its band list those pairs (a warp-level exclusive scan assigns the slots).
+KGE_DEV void tc_epilogue(const float (&acc)[64], const float (&nl)[32], const TcBand (&Bq)[2], int64_t qa, int64_t cbase,
+                         int nvalid, const TcParams& P, const TcDirView& V, TcListState& L, int lane, int (&cnt)[2]) {
+  const int cl = 2 * (lane & 3);
+  int amb = 0;
 #pragma unroll
-    for (int j = 0; j < 32; j += 2) {
-      TC_CMP(hi0, lo0, __uint_as_float(v[j]), j);
-      TC_CMP(hi1, lo1, __uint_as_float(v[j + 1]), j + 1);
-    }
-  } else {
+  for (int j = 0; j < 16; ++j) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const float nj = __shfl_sync(0xffffffffu, nl, j);   // (all lanes take part; columns >= nv are skipped)
-      if (j < nv) {
-        float u_, h_;
-        tc_band_eval(Bq, __uint_as_float(v[j]), nj, u_, h_);
-        hi0 += (u_ > h_) ? 1 : 0;
-        lo0 += (u_ >= -h_) ? 1 : 0;
+    for (int c = 0; c < 2; ++c) {
+      const bool ok = 8 * j + cl + c < nvalid;
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        float u, h;
+        tc_band_eval(Bq[i], acc[4 * j + 2 * i + c], nl[2 * j + c], u, h);
+        cnt[i] += (ok && u > h) ? 1 : 0;
+        amb += (ok && u >= -h && !(u > h)) ? 1 : 0;
       }
     }
   }
-#undef TC_CMP
-  const int hi = hi0 + hi1;
-  const int na = (lo0 + lo1) - hi;   // this row's candidates inside the band
-  if (stamp) TC_STAMP(2, ev++);
-  if (P.epi_mode != 2 && __any_sync(0xffffffffu, na != 0)) {
-    // Transpose the band predicate with one vote per column: lane j ends up with the mask of the ROWS whose
-    // candidate cbase+j is ambiguous, so every lane lists its own column's pairs with no divergent code in the
-    // 32-column loop (the per-row form — 32 predicated stores per thread — cost 2-4k cycles per event:
-    // profiles/r2_tc_trace_v9_globalmax.jsonl).
-    unsigned mine = 0u;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const float nj = __shfl_sync(0xffffffffu, nl, j);
-      float u_, h_;
-      tc_band_eval(Bq, __uint_as_float(v[j]), nj, u_, h_);
-      const unsigned m = __ballot_sync(0xffffffffu, j < nv && u_ >= -h_ && !(u_ > h_));
-      if (lane == j) mine = m;
-    }
-    const int mycnt = __popc(mine);
-    int incl = mycnt;
+  if (P.epi_mode != 2 && __any_sync(0xffffffffu, amb != 0)) {
+    int incl = amb;
 #pragma unroll
     for (int off = 1; off < 32; off <<= 1) {
       const int t = __shfl_up_sync(0xffffffffu, incl, off);
@@ -301,39 +219,50 @@ KGE_DEV int tc_scan_chunk(const uint32_t (&v)[32], int nv, const TcBand& Bq, flo
       tc_list_pad(L, P, V, lane);
       tc_list_reserve(L, P, V, lane, total > kTcListBlock ? total : kTcListBlock);
     }
-    unsigned k = L.base + L.used + (unsigned)(incl - mycnt);
-    const int64_t qrow0 = q - lane;   // the warp's rows are consecutive queries
-    while (mine) {
-      const int r = __ffs((int)mine) - 1;
-      mine &= mine - 1u;
-      if (k < P.cap) V.list[k] = ((unsigned long long)(qrow0 + r) << 32) | (unsigned long long)(cbase + lane);
-      ++k;
+    unsigned k = L.base + L.used + (unsigned)(incl - amb);
+    if (amb) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int col = 8 * j + cl + c;
+#pragma unroll
+          for (int i = 0; i < 2; ++i) {
+            float u, h;
+            tc_band_eval(Bq[i], acc[4 * j + 2 * i + c], nl[2 * j + c], u, h);
+            if (col < nvalid && u >= -h && !(u > h)) {
+              if (k < P.cap) V.list[k] = ((unsigned long long)(qa + 8 * i) << 32) | (unsigned long long)(cbase + col);
+              ++k;
+            }
+          }
+        }
+      }
     }
     L.used += total;
   }
-  if (V.dbg && live) {
+  if (V.dbg) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j)
-      if (j < nv) V.dbg[(size_t)q * (size_t)P.nc + (size_t)(cbase + j)] = __uint_as_float(v[j]);
+    for (int i = 0; i < 2; ++i) {
+      const int64_t q = qa + 8 * i;
+      if (q >= P.Q) continue;
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c)
+          if (8 * j + cl + c < nvalid) V.dbg[(size_t)q * (size_t)P.nc + (size_t)(cbase + 8 * j + cl + c)] = acc[4 * j + 2 * i + c];
+    }
   }
-  return hi;
 }
 
 // ---- the sweep ------------------------------------------------------------------------------------
-// grid (splits, query blocks); CTA = 128 queries x a run of 128-candidate tiles.
-//   warp 0 lane 0 : TMA producer (query k-blocks once when they fit, candidate k-blocks through a
-//                   ring of stages)
-//   warp 1 lane 0 : issues the tcgen05.mma chain of a tile into accumulator stage t&1; tcgen05.commit
-//                   releases smem stages and publishes finished accumulators
-//   warps 2..9    : epilogue — warp w owns TMEM lanes 32*(w&3).. (= query rows) and the column half
-//                   (w-2)/4 of the tile (= 64 candidates), 32 columns per tcgen05.ld, each compared with the
-//                   band of its (query, candidate) pair
-// PAIR: launched as clusters of two CTAs (1 x 2 x 1: same candidate tiles, adjacent query blocks).  Each CTA
-// issues the TMA loads of HALF of every candidate k-block (64 of its 128 rows) and multicasts them into both
-// CTAs' stages, so an SM requests half the rows and the L2 is read once per pair (a test of the hypothesis that
-// the L2->SM operand stream sets the k-block cadence: it does not, see tc_sweep()).  A stage is refilled only when the
-// MMAs of BOTH CTAs have consumed it (tcgen05.commit multicast onto both empty barriers, count 2).
-template <bool PAIR>
+// grid (splits, query blocks, directions); CTA = 128 queries x a run of 128-candidate tiles.
+//   warpgroup 0, thread 0 : TMA producer (query k-blocks once when they fit, riding on the first tile's
+//                           stages; candidate k-blocks — and streamed query k-blocks — through a ring of stages)
+//   warpgroups 1, 2       : query rows [0, 64) / [64, 128) of the block.  Per k-block 3 x (Kp/16 per block)
+//                           wgmma into 64 fp32 registers per thread; a stage is released (one arrive per warp on
+//                           its empty barrier) once the wgmma group that read it has retired; after the tile's
+//                           last k-block the warpgroup runs the band epilogue on its registers while the producer
+//                           keeps filling stages for the next tile.
 __global__ void __launch_bounds__(kTcThreads, 1)
 tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMaps TM) {
   extern __shared__ unsigned char tc_smem_raw[];
@@ -343,28 +272,22 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
   const uint32_t raw = tc_smem_u32(tc_smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B tiles need 1024-byte alignment
   unsigned char* const gbase = tc_smem_raw + (base - raw);
-  uint64_t* const bars = reinterpret_cast<uint64_t*>(gbase);    // control block: first 1024 bytes
-  uint64_t* const full = bars;                                  // [kTcMaxStages]
-  uint64_t* const empty = bars + kTcMaxStages;                  // [kTcMaxStages]
-  uint64_t* const a_full = bars + 2 * kTcMaxStages;             // [1]
-  uint64_t* const tmem_full = a_full + 1;                       // [2]
-  uint64_t* const tmem_empty = tmem_full + 2;                   // [2]
-  uint32_t* const tmem_slot = reinterpret_cast<uint32_t*>(gbase + 512);
-  const uint32_t a_base = base + 1024u;                                            // resident query k-blocks
-  const uint32_t a_bytes = (!P.a_resident || P.a_tmem) ? 0u
-      : (P.tail_cols ? (uint32_t)(P.nkb - 1) * 2u * P.tile_bytes + 2u * P.tail_bytes : (uint32_t)P.nkb * 2u * P.tile_bytes);
+  uint64_t* const full = reinterpret_cast<uint64_t*>(gbase);    // control block: first 1024 bytes
+  uint64_t* const empty = full + kTcMaxStages;
+  const uint32_t a_base = base + 1024u;                         // resident query k-blocks
+  const uint32_t tb = P.tile_bytes;
+  const uint32_t a_bytes = P.a_resident ? (uint32_t)P.nkb * 2u * tb : 0u;
   const uint32_t st_base = a_base + a_bytes;
-  const uint32_t st_bytes = (P.a_resident ? 2u : 4u) * P.tile_bytes;              // [B0][B1]([A0][A1])
+  const uint32_t st_bytes = (P.a_resident ? 2u : 4u) * tb;     // [B0][B1]([A0][A1])
 
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);
   const int lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
   const int64_t q0 = (int64_t)blockIdx.y * kTcBM;
   const bool zdir = blockIdx.z != 0;
   const TcDirView& V = zdir ? P.D[1] : P.D[0];
   const CUtensorMap* const ma0 = zdir ? &TM.c0 : &TM.a0;
   const CUtensorMap* const ma1 = zdir ? &TM.c1 : &TM.a1;
-  const CUtensorMap* const ma0t = zdir ? &TM.c0t : &TM.a0t;
-  const CUtensorMap* const ma1t = zdir ? &TM.c1t : &TM.a1t;
   if (threadIdx.x == 0) TC_STAMP(2, 63);   // kernel entry of CTA (0,0)
   // wall-clock span of EVERY CTA (%globaltimer, ns) behind the three role timelines: launch skew and stragglers
   const unsigned cta_lin = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
@@ -375,199 +298,127 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
   }
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < P.nstages; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], PAIR ? 2 : 1); }
-    tc_mbar_init(a_full, P.a_tmem ? (uint32_t)kTcEpiWarps : 1u);
-    for (int s = 0; s < 2; ++s) { tc_mbar_init(&tmem_full[s], 1); tc_mbar_init(&tmem_empty[s], kTcEpiWarps); }
+    for (int s = 0; s < P.nstages; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], kTcConsumerWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) {   // TMEM allocation is warp-collective; the same warp frees it
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                 ::"r"(tc_smem_u32(tmem_slot)), "r"((uint32_t)(P.a_tmem ? 2 * kTcTmemCols : kTcTmemCols)) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  if (PAIR) tc_cluster_sync();   // the peer's barriers exist before anything of ours can reach them
-  const uint32_t tmem_base = *reinterpret_cast<volatile uint32_t*>(tmem_slot);
-  const uint32_t crank = PAIR ? (blockIdx.y & 1u) : 0u;   // rank in the (1,2,1) cluster
 
-  if (warp == 0) {
-    if (lane == 0) {
-      // (resident query k-blocks ride on the FIRST tile's stage barriers, k-block by k-block: the first MMA needs
-      // 64 KB in shared memory, not the whole query block + three stages — see the loop below)
-      const bool a_with_first_tile = P.a_resident && !P.a_tmem;
+  if (wg == 0) {
+    // the producer needs few registers: hand them to the consumers' 64 accumulators + 32 norm bounds
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;" ::: "memory");
+    if (threadIdx.x == 0) {
       int stage = 0; uint32_t phase = 0;
       int ev = 0;
       TC_STAMP(0, ev++);
       for (int t = 0; t < ntl; ++t) {
         const int row = (t0 + t) * kTcBN;
         for (int kb = 0; kb < P.nkb; ++kb) {
-          const bool tail = P.tail_cols && kb == P.nkb - 1;
-          const uint32_t tb = tail ? P.tail_bytes : P.tile_bytes;
           tc_mbar_wait(&empty[stage], phase ^ 1u);
           TC_STAMP(0, ev++);
-          const bool with_a = a_with_first_tile && t == 0;
+          // resident query k-blocks ride on the FIRST tile's stage barriers, k-block by k-block: the first wgmma
+          // needs one k-block of each operand in shared memory, not the whole query block
+          const bool with_a = P.a_resident && t == 0;
           tc_mbar_expect_tx(&full[stage], ((P.a_resident && !with_a) ? 2u : 4u) * tb);
           const uint32_t sb = st_base + (uint32_t)stage * st_bytes;
+          const int col = kb * kTcBK;
           if (with_a) {
-            const uint32_t dst = a_base + (uint32_t)kb * 2u * P.tile_bytes;
-            tc_tma_load_2d(dst, tail ? ma0t : ma0, kb * P.bk, (int)q0, &full[stage]);
-            tc_tma_load_2d(dst + tb, tail ? ma1t : ma1, kb * P.bk, (int)q0, &full[stage]);
+            const uint32_t dst = a_base + (uint32_t)kb * 2u * tb;
+            tc_tma_load_2d(dst, ma0, col, (int)q0, &full[stage]);
+            tc_tma_load_2d(dst + tb, ma1, col, (int)q0, &full[stage]);
           }
-          if (PAIR) {   // my half of the candidate rows, into both CTAs (the peer sends the other half)
-            const uint32_t ho = crank * (tb >> 1);
-            const int hrow = row + (int)crank * (kTcBN / 2);
-            tc_tma_load_2d_mc(sb + ho, tail ? &TM.b0t : &TM.b0, kb * P.bk, hrow, &full[stage], (uint16_t)3);
-            tc_tma_load_2d_mc(sb + tb + ho, tail ? &TM.b1t : &TM.b1, kb * P.bk, hrow, &full[stage], (uint16_t)3);
-          } else {
-            tc_tma_load_2d(sb, tail ? &TM.b0t : &TM.b0, kb * P.bk, row, &full[stage]);
-            tc_tma_load_2d(sb + tb, tail ? &TM.b1t : &TM.b1, kb * P.bk, row, &full[stage]);
-          }
+          tc_tma_load_2d(sb, &TM.b0, col, row, &full[stage]);
+          tc_tma_load_2d(sb + tb, &TM.b1, col, row, &full[stage]);
           if (!P.a_resident) {
-            tc_tma_load_2d(sb + 2u * tb, tail ? ma0t : ma0, kb * P.bk, (int)q0, &full[stage]);
-            tc_tma_load_2d(sb + 3u * tb, tail ? ma1t : ma1, kb * P.bk, (int)q0, &full[stage]);
+            tc_tma_load_2d(sb + 2u * tb, ma0, col, (int)q0, &full[stage]);
+            tc_tma_load_2d(sb + 3u * tb, ma1, col, (int)q0, &full[stage]);
           }
-          if (++stage == P.nstages) { stage = 0; phase ^= 1u; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      int ev = 0;
-      TC_STAMP(1, ev++);
-      if (P.a_tmem) { tc_mbar_wait(a_full, 0u); tc_fence_after(); }   // (smem-resident query blocks arrive with the first tile's stages)
-      TC_STAMP(1, ev++);
-      int stage = 0; uint32_t phase = 0;
-      for (int t = 0; t < ntl; ++t) {
-        const int as = t & 1;
-        tc_mbar_wait(&tmem_empty[as], (uint32_t)(((t >> 1) & 1) ^ 1));   // epilogue has drained this accumulator
-        tc_fence_after();
-        TC_STAMP(1, ev++);
-        const uint32_t d_tmem = tmem_base + (uint32_t)(as * kTcBN);
-        for (int kb = 0; kb < P.nkb; ++kb) {
-          tc_mbar_wait(&full[stage], phase);
-          tc_fence_after();
-          TC_STAMP(1, ev++);
-          const bool tail = P.tail_cols && kb == P.nkb - 1;
-          const uint32_t tb = tail ? P.tail_bytes : P.tile_bytes;
-          const uint32_t rowb = tail ? (uint32_t)P.tail_cols * 2u : (uint32_t)P.bk * 2u;   // bytes per smem row = swizzle span
-          const uint32_t sb = st_base + (uint32_t)stage * st_bytes;
-          const uint32_t b0 = sb, b1 = sb + tb;
-          const uint32_t a0 = P.a_resident ? a_base + (uint32_t)kb * 2u * P.tile_bytes : sb + 2u * tb;
-          const uint32_t a1 = a0 + tb;
-          const int nks = tail ? P.tail_cols / 16 : min(P.bk / 16, (P.Kp - kb * P.bk + 15) / 16);
-          const uint64_t da0 = tc_smem_desc(a0, rowb), da1 = tc_smem_desc(a1, rowb), db0 = tc_smem_desc(b0, rowb),
-                         db1 = tc_smem_desc(b1, rowb);
-          if (P.a_tmem) {
-            // query operands in tensor memory: a0 at columns [256, 256 + Kp/2), a1 right behind; a k-step is 8 columns
-            const uint32_t ta0 = tmem_base + (uint32_t)(2 * kTcBN) + (uint32_t)((kb * P.bk) >> 1);
-            const uint32_t ta1 = ta0 + (uint32_t)(P.Kp >> 1);
-            for (int k = 0; k < nks; ++k) {
-              const uint64_t ko = (uint64_t)(2 * k);
-              tc_mma_ts(d_tmem, ta0 + 8u * k, db0 + ko, kTcIdesc, (kb | k) != 0 ? 1u : 0u);
-              tc_mma_ts(d_tmem, ta0 + 8u * k, db1 + ko, kTcIdesc, 1u);
-              tc_mma_ts(d_tmem, ta1 + 8u * k, db0 + ko, kTcIdesc, 1u);
-            }
-          } else
-          for (int k = 0; k < nks; ++k) {   // 16 bf16 = 32 bytes further along the swizzled row: +2 in the address field
-            const uint64_t ko = (uint64_t)(2 * k);
-            tc_mma(d_tmem, da0 + ko, db0 + ko, kTcIdesc, (kb | k) != 0 ? 1u : 0u);
-            tc_mma(d_tmem, da0 + ko, db1 + ko, kTcIdesc, 1u);
-            tc_mma(d_tmem, da1 + ko, db0 + ko, kTcIdesc, 1u);
-          }
-          if (PAIR) tc_commit_mc(&empty[stage], (uint16_t)3);   // both CTAs' producers write this stage: tell both
-          else tc_commit(&empty[stage]);                    // smem stage reusable once these MMAs are done
-          if (kb == P.nkb - 1) tc_commit(&tmem_full[as]);   // ... and the accumulator is complete
           if (++stage == P.nstages) { stage = 0; phase ^= 1u; }
         }
       }
     }
   } else {
-    const int quad = warp & 3;                 // TMEM lane quadrant this warp may access
-    const int row = quad * 32 + lane;
-    const int64_t q = q0 + row;
-    const bool live = q < P.Q;
-    TcBand Bq = {INFINITY, 0.f, 0.f, 0.f};   // rows beyond Q: u = -inf -> nothing counted, nothing listed
-    if (live) {
-      const float4 tq = __ldg(reinterpret_cast<const float4*>(V.tau) + q);
-      Bq.centre = tq.x; Bq.a = tq.y; Bq.b = tq.z; Bq.e = tq.w;
-    }
-    if (P.a_tmem) {
-      // this thread's query row -> tensor memory: warps 2-5 write the high parts a0, warps 6-9 the low parts a1;
-      // a row is Kp bf16 = Kp/2 32-bit columns (two consecutive k per column), rows beyond Q are zeros
-      const int half = (warp - 2) >> 2;
-      const __nv_bfloat16* src = (half == 0 ? V.A0 : V.A1) + (size_t)(live ? q : 0) * P.Kp;
-      const uint32_t tdst = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(2 * kTcBN) + (uint32_t)(half * (P.Kp >> 1));
-      for (int c = 0; c < (P.Kp >> 1); c += 8) {   // Kp is a multiple of 16: whole groups of 8 columns
-        uint4 lo = make_uint4(0u, 0u, 0u, 0u), hi = lo;
-        if (live) {
-          lo = __ldg(reinterpret_cast<const uint4*>(src + 2 * c));
-          hi = __ldg(reinterpret_cast<const uint4*>(src + 2 * c + 8));
-        }
-        const uint32_t v[8] = {lo.x, lo.y, lo.z, lo.w, hi.x, hi.y, hi.z, hi.w};
-        tc_tmem_st8(tdst + (uint32_t)c, v);
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;" ::: "memory");
+    const int half = wg - 1;                               // query rows [64 half, 64 half + 64) of the block
+    const int64_t qa = q0 + 64 * half + 16 * (warp & 3) + (lane >> 2);   // this thread's rows: qa, qa + 8
+    TcBand Bq[2];
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      const int64_t q = qa + 8 * i;
+      Bq[i] = {INFINITY, 0.f, 0.f, 0.f};                   // rows beyond Q: u = -inf -> nothing counted, nothing listed
+      if (q < P.Q) {
+        const float4 tq = __ldg(reinterpret_cast<const float4*>(V.tau) + q);
+        Bq[i] = {tq.x, tq.y, tq.z, tq.w};
       }
-      tc_tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) tc_mbar_arrive(a_full);
     }
-    int cnt = 0;
+    const uint32_t a_off = (uint32_t)half * 64u * (uint32_t)(kTcBK * 2);   // 64 rows of 128 bytes into the A tile
+    int cnt[2] = {0, 0};
     TcListState L = {0u, 0u, 0u};
     tc_list_reserve(L, P, V, lane, kTcListBlock);   // the warp's first block: the atomic's round trip hides behind the first tile's MMAs
+    const bool stamper = warp == 4 && lane == 0;
     int ev = 0;
-    if (warp == 2 && lane == 0) TC_STAMP(2, ev++);
+    if (stamper) TC_STAMP(1, ev++);
+    int stage = 0; uint32_t phase = 0;
+    float acc[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    float nl[32];
     for (int t = 0; t < ntl; ++t) {
-      const int as = t & 1;
       const int64_t cbase = (int64_t)(t0 + t) * kTcBN;
-      // this warp's half of the tile's columns: [c0, c0 + 64)
-      const int c0 = ((warp - 2) >> 2) * (kTcBN / 2);
-      // the candidates' norm bounds for the two 32-column chunks (lane = column), requested before the
-      // wait for the accumulator so that the L2 latency is off the path
-      const int64_t ca = cbase + c0 + lane, cb2 = ca + 32;
-      const float nla = ca < P.nc ? __ldg(P.cn + ca) : 0.f;
-      const float nlb = cb2 < P.nc ? __ldg(P.cn + cb2) : 0.f;
-      tc_mbar_wait(&tmem_full[as], (uint32_t)((t >> 1) & 1));
-      tc_fence_after();
-      if (warp == 2 && lane == 0) TC_STAMP(2, ev++);
       const int nvalid = (int)min((int64_t)kTcBN, P.nc - cbase);
-      const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + (uint32_t)(as * kTcBN);
-      const int nloc = min(kTcBN / 2, nvalid - c0);          // valid columns in the half (may be <= 0)
-      const int nchunks = nloc > 0 ? (nloc + 31) >> 5 : 0;   // 0, 1 or 2
-      // two register buffers: the tcgen05.ld of chunk 1 is in flight while chunk 0 is compared
-      uint32_t va[32], vb[32];
-      if (nchunks > 0) {
-        tc_tmem_ld32(taddr + (uint32_t)c0, va);
-        tc_tmem_wait_ld();
-        if (nchunks > 1) tc_tmem_ld32(taddr + (uint32_t)(c0 + 32), vb);
-        cnt += tc_scan_chunk(va, min(32, nloc), Bq, nla, q, cbase + c0, live, P, V, L, lane, ev, warp == 2 && lane == 0);
-        if (nchunks > 1) {
-          tc_tmem_wait_ld();
-          cnt += tc_scan_chunk(vb, min(32, nloc - 32), Bq, nlb, q, cbase + c0 + 32, live, P, V, L, lane, ev, warp == 2 && lane == 0);
+      // the candidates' norm bounds of this thread's 32 columns, requested before the MMAs so that the L2
+      // latency is off the path
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+#pragma unroll
+        for (int c = 0; c < 2; ++c) {
+          const int col = 8 * j + 2 * (lane & 3) + c;
+          nl[2 * j + c] = col < nvalid ? __ldg(P.cn + cbase + col) : 0.f;
         }
+      int prev = -1;
+      for (int kb = 0; kb < P.nkb; ++kb) {
+        tc_mbar_wait(&full[stage], phase);
+        const uint32_t sb = st_base + (uint32_t)stage * st_bytes;
+        const uint32_t a0 = (P.a_resident ? a_base + (uint32_t)kb * 2u * tb : sb + 2u * tb) + a_off;
+        const uint64_t da0 = tc_smem_desc(a0), da1 = tc_smem_desc(a0 + tb);
+        const uint64_t db0 = tc_smem_desc(sb), db1 = tc_smem_desc(sb + tb);
+        const int nks = min(kTcBK / 16, (P.Kp - kb * kTcBK) / 16);   // Kp is a multiple of 16; columns past it are TMA zero fill
+        tc_wgmma_fence();
+#pragma unroll 1
+        for (int k = 0; k < nks; ++k) {
+          const uint64_t ko = (uint64_t)(2 * k);
+          tc_wgmma(acc, da0 + ko, db0 + ko, (kb | k) != 0 ? 1u : 0u);
+          tc_wgmma(acc, da0 + ko, db1 + ko, 1u);
+          tc_wgmma(acc, da1 + ko, db0 + ko, 1u);
+        }
+        tc_wgmma_commit();
+        tc_wgmma_wait<1>();   // the group of the previous k-block has retired: its stage may be refilled
+        if (prev >= 0) { __syncwarp(); if (lane == 0) tc_mbar_arrive(&empty[prev]); }
+        prev = stage;
+        if (++stage == P.nstages) { stage = 0; phase ^= 1u; }
       }
-      tc_fence_before();
+      tc_wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) tc_mbar_arrive(&tmem_empty[as]);
-      if (warp == 2 && lane == 0) TC_STAMP(2, ev++);
+      if (lane == 0) tc_mbar_arrive(&empty[prev]);
+      if (stamper) TC_STAMP(2, ev++);
+      if (P.epi_mode != 1) tc_epilogue(acc, nl, Bq, qa, cbase, nvalid, P, V, L, lane, cnt);
+      if (stamper) TC_STAMP(2, ev++);
     }
     tc_list_pad(L, P, V, lane);   // the unused slots of the warp's last block become holes
-    if (live && cnt) atomicAdd(V.tc_counts + q, cnt);
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {   // the four lanes of a row hold its 32 columns each
+      cnt[i] += __shfl_xor_sync(0xffffffffu, cnt[i], 1);
+      cnt[i] += __shfl_xor_sync(0xffffffffu, cnt[i], 2);
+      const int64_t q = qa + 8 * i;
+      if ((lane & 3) == 0 && q < P.Q && cnt[i]) atomicAdd(V.tc_counts + q, cnt[i]);
+    }
   }
-  tc_fence_before();
   __syncthreads();
   if (P.trace && threadIdx.x == 0 && cta_lin < 1024u) {
     unsigned long long ns;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(ns));
     P.trace[192 + 2 * cta_lin + 1] = (long long)ns;
     if (cta_lin == 0) P.trace[2 * 64 + 62] = clock64();   // CTA (0,0,0): cycles at exit, next to its ns span
-  }
-  if (PAIR) tc_cluster_sync();   // neither CTA leaves while the peer can still multicast into it / arrive on its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"((uint32_t)(P.a_tmem ? 2 * kTcTmemCols : kTcTmemCols)) : "memory");
   }
 }
 
@@ -655,7 +506,7 @@ bool tc_supported(const kge_model_t* m, int64_t nc) {
 
 unsigned tc_list_capacity(int64_t Q) {
   int64_t cap = 512 * Q;
-  if (cap < 32768) cap = 32768;   // (every epilogue warp reserves one block of 16 up front: <= 148 x 8 x 16 slots)
+  if (cap < 32768) cap = 32768;   // (every consumer warp reserves one block of 16 up front: <= one wave of CTAs x 8 x 16 slots)
   if (cap > (1 << 24)) cap = 1 << 24;
   return (unsigned)cap;
 }
@@ -700,18 +551,15 @@ static TcEncodeFn tc_encode_fn() {
   return fn;
 }
 // bf16 matrix [rows][Kp] row-major; box = {64 columns (128 bytes), 128 rows}, 128-byte swizzle, zero fill
-// (box_cols = 64: one 128-byte swizzle row; 32 / 16: the narrow tile of an exact-width last k-block)
-static int tc_make_map(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t Kp, int box_cols, int box_rows = kTcBN) {
+static int tc_make_map(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t Kp) {
   TcEncodeFn fn = tc_encode_fn();
   if (!fn) { set_error("cuTensorMapEncodeTiled is not available"); return KGE_ECUDA; }
   const cuuint64_t gdim[2] = {Kp, rows};
   const cuuint64_t gstride[1] = {Kp * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+  const cuuint32_t box[2] = {(cuuint32_t)kTcBK, (cuuint32_t)kTcBN};
   const cuuint32_t estr[2] = {1, 1};
-  const CUtensorMapSwizzle sw = box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B
-                              : (box_cols == 32 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_32B);
   const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (bf16) failed (%d)", (int)r); return KGE_ECUDA; }
   return KGE_OK;
@@ -791,34 +639,15 @@ int tc_sweep(const kge_model_t* m, int dir, int ndirs, int64_t Q, int64_t nc, vo
     const TcQueryArgs T = tc_query_args(m, dz, tcws, Q);
     P.D[z].tau = T.tau; P.D[z].tc_counts = T.tc_counts; P.D[z].ctrl = T.ctrl;
     P.D[z].list = reinterpret_cast<unsigned long long*>(w + L.list[dz]);
-    P.D[z].A0 = T.A0; P.D[z].A1 = T.A1; P.D[z].dbg = (z == 0) ? dbg : nullptr;
+    P.D[z].dbg = (z == 0) ? dbg : nullptr;
     A0[z] = T.A0; A1[z] = T.A1;
   }
   P.cn = reinterpret_cast<const float*>(w + L.cn); P.cap = tc_list_capacity(Q);
-  // k-block width: 64 columns (128-byte swizzle rows).  32-column blocks (64-byte rows) would give 7 pipeline
-  // stages instead of 3, but measured SLOWER (26.6 vs 24.5 us, profiles/r2_tc_trace_v6.jsonl): prefetch depth is
-  // not what limits the k-block cadence.  KGE_TC_BK=32 keeps the variant reachable for tests.
-  int bk = 64;
-  if (const char* e = getenv("KGE_TC_BK")) { if (atoi(e) == 32) bk = 32; }   // tuning / test aid
-  P.bk = bk;
-  P.tile_bytes = (uint32_t)(kTcBN * bk * 2);
-  P.Q = Q; P.nc = nc; P.Kp = Kp; P.nkb = (Kp + bk - 1) / bk;
+  P.tile_bytes = (uint32_t)(kTcBN * kTcBK * 2);
+  P.Q = Q; P.nc = nc; P.Kp = Kp; P.nkb = (Kp + kTcBK - 1) / kTcBK;
   P.a_resident = Kp <= kTcResidentMaxK ? 1 : 0;
-  {
-    const int last = Kp - bk * (P.nkb - 1);   // columns of the last k-block: a multiple of 16 up to bk
-    P.tail_cols = (last < bk && (last == 16 || last == 32)) ? last : 0;
-    if (const char* e = getenv("KGE_TC_TAIL")) { if (atoi(e) == 0) P.tail_cols = 0; }   // tuning / test aid
-    P.tail_bytes = (uint32_t)(kTcBN * P.tail_cols * 2);
-  }
-  // query operands in tensor memory (KGE_TC_ATMEM=1; they fit beside the two accumulators when 2 x Kp/2 <= 256
-  // columns): halves the shared-memory reads of an MMA and frees 104 KB for 7 candidate stages.  Correct (tests
-  // run both) but measured slower (26.6 vs 24.6 us): the per-thread fill of tensor memory costs ~5 us of prologue
-  // and the MMA cadence does not change — the query operand's shared-memory reads alone are not the limiter either.
-  P.a_tmem = 0;
-  if (const char* e = getenv("KGE_TC_ATMEM")) { if (atoi(e) != 0 && P.a_resident && Kp <= 256) P.a_tmem = 1; }
-  const size_t budget = 227 * 1024 - 2048;   // control block + alignment slack
-  const size_t a_bytes = (!P.a_resident || P.a_tmem) ? 0
-      : (P.tail_cols ? (size_t)(P.nkb - 1) * 2 * P.tile_bytes + 2 * (size_t)P.tail_bytes : (size_t)P.nkb * 2 * P.tile_bytes);
+  const size_t budget = 227 * 1024 - 2048;   // opt-in shared memory of a block on sm_90, minus control block + alignment slack
+  const size_t a_bytes = P.a_resident ? (size_t)P.nkb * 2 * P.tile_bytes : 0;
   const size_t st_bytes = (P.a_resident ? 2 : 4) * (size_t)P.tile_bytes;
   int nstages = (int)((budget - a_bytes) / st_bytes);
   if (nstages > kTcMaxStages) nstages = kTcMaxStages;
@@ -835,54 +664,19 @@ int tc_sweep(const kge_model_t* m, int dir, int ndirs, int64_t Q, int64_t nc, vo
   P.trace = g_tc_trace;
   P.epi_mode = 0;
   if (const char* e = getenv("KGE_TC_EPI_MODE")) P.epi_mode = atoi(e);   // measurement aid: wrong counts unless 0
-  // pair mode (KGE_TC_PAIR=1): two query blocks share every candidate tile through TMA multicast.  Correct
-  // (tests run both) but measured NOT faster (24.6 vs 22.5-24.6 us, profiles/r2_tc_trace_v7_pair.jsonl,
-  // r2_tc_trace_v8_modes.txt): halving the L2->SM stream does not move the k-block cadence (~100 cycles per
-  // 128x128x16 tcgen05.mma while the tensor pipe is busy ~56 of them: DESIGN.md 5b "What bounds it").
-  bool pair = false;
-  if (const char* e = getenv("KGE_TC_PAIR")) pair = atoi(e) != 0;
-  const int brows = pair ? kTcBN / 2 : kTcBN;
   TcMaps TM;
-  int rc = tc_make_map(&TM.a0, A0[0], (uint64_t)Q, (uint64_t)Kp, bk); if (rc) return rc;
-  rc = tc_make_map(&TM.a1, A1[0], (uint64_t)Q, (uint64_t)Kp, bk); if (rc) return rc;
-  rc = tc_make_map(&TM.c0, A0[1], (uint64_t)Q, (uint64_t)Kp, bk); if (rc) return rc;
-  rc = tc_make_map(&TM.c1, A1[1], (uint64_t)Q, (uint64_t)Kp, bk); if (rc) return rc;
-  rc = tc_make_map(&TM.b0, w + L.b[0], (uint64_t)nc, (uint64_t)Kp, bk, brows); if (rc) return rc;
-  rc = tc_make_map(&TM.b1, w + L.b[1], (uint64_t)nc, (uint64_t)Kp, bk, brows); if (rc) return rc;
-  TM.a0t = TM.a0; TM.a1t = TM.a1; TM.b0t = TM.b0; TM.b1t = TM.b1; TM.c0t = TM.c0; TM.c1t = TM.c1;
-  if (P.tail_cols) {
-    rc = tc_make_map(&TM.a0t, A0[0], (uint64_t)Q, (uint64_t)Kp, P.tail_cols); if (rc) return rc;
-    rc = tc_make_map(&TM.a1t, A1[0], (uint64_t)Q, (uint64_t)Kp, P.tail_cols); if (rc) return rc;
-    rc = tc_make_map(&TM.c0t, A0[1], (uint64_t)Q, (uint64_t)Kp, P.tail_cols); if (rc) return rc;
-    rc = tc_make_map(&TM.c1t, A1[1], (uint64_t)Q, (uint64_t)Kp, P.tail_cols); if (rc) return rc;
-    rc = tc_make_map(&TM.b0t, w + L.b[0], (uint64_t)nc, (uint64_t)Kp, P.tail_cols, brows); if (rc) return rc;
-    rc = tc_make_map(&TM.b1t, w + L.b[1], (uint64_t)nc, (uint64_t)Kp, P.tail_cols, brows); if (rc) return rc;
-  }
+  int rc = tc_make_map(&TM.a0, A0[0], (uint64_t)Q, (uint64_t)Kp); if (rc) return rc;
+  rc = tc_make_map(&TM.a1, A1[0], (uint64_t)Q, (uint64_t)Kp); if (rc) return rc;
+  rc = tc_make_map(&TM.c0, A0[1], (uint64_t)Q, (uint64_t)Kp); if (rc) return rc;
+  rc = tc_make_map(&TM.c1, A1[1], (uint64_t)Q, (uint64_t)Kp); if (rc) return rc;
+  rc = tc_make_map(&TM.b0, w + L.b[0], (uint64_t)nc, (uint64_t)Kp); if (rc) return rc;
+  rc = tc_make_map(&TM.b1, w + L.b[1], (uint64_t)nc, (uint64_t)Kp); if (rc) return rc;
   const size_t smem = 2048 + a_bytes + (size_t)nstages * st_bytes;
   SweepProfile* sp = sweep_profile(dir);
-  if (pair) {
-    // clusters of (1, 2, 1): the grid's query-block dimension is padded to an even count (a padding CTA has
-    // no live rows: its operand rows arrive zero-filled, its thresholds are +inf, it only relays its half loads)
-    const unsigned qb2 = (unsigned)((qblocks + 1) & ~1);
-    KGE_CUDA_OK(cudaFuncSetAttribute(tc_sweep_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((unsigned)splits, qb2, (unsigned)ndirs);
-    cfg.blockDim = dim3(kTcThreads, 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 1; attr[0].val.clusterDim.y = 2; attr[0].val.clusterDim.z = 1;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    if (sp->armed) KGE_CUDA_OK(cudaEventRecord(sp->beg, st));
-    KGE_CUDA_OK(cudaLaunchKernelEx(&cfg, tc_sweep_kernel<true>, P, TM));
-    KGE_CHECK_LAUNCH("tc_sweep_kernel<pair>");
-  } else {
-    KGE_CUDA_OK(cudaFuncSetAttribute(tc_sweep_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    if (sp->armed) KGE_CUDA_OK(cudaEventRecord(sp->beg, st));
-    tc_sweep_kernel<false><<<dim3((unsigned)splits, (unsigned)qblocks, (unsigned)ndirs), kTcThreads, smem, st>>>(P, TM);
-    KGE_CHECK_LAUNCH("tc_sweep_kernel");
-  }
+  KGE_CUDA_OK(cudaFuncSetAttribute(tc_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  if (sp->armed) KGE_CUDA_OK(cudaEventRecord(sp->beg, st));
+  tc_sweep_kernel<<<dim3((unsigned)splits, (unsigned)qblocks, (unsigned)ndirs), kTcThreads, smem, st>>>(P, TM);
+  KGE_CHECK_LAUNCH("tc_sweep_kernel");
   if (sp->armed) { KGE_CUDA_OK(cudaEventRecord(sp->end, st)); sp->valid = true; sp->ndirs = ndirs; }
   return KGE_OK;
 }

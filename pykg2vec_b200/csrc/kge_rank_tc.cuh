@@ -82,8 +82,7 @@ KGE_DEV float tc_sqrt_domain_threshold(float th) {
 // Every term is a polynomial of degree <= 2 in n with per-query coefficients, so the epilogue evaluates
 // half(q,c) = a + b n + e n^2 with two fma (r2 first used max_c|c| for n: exact too, but one heavy row —
 // trained tables have them — widened every pair's band; now the band of a pair scales with ITS candidate).
-// Measured on the B200 (tests/test_gpu_baseline_shapes.py, profiles/r2_tc_parity.jsonl): the real error is
-// 35x (d = 200) to 400x (d = 1000) below this bound.
+// tests/test_gpu_baseline_shapes.py measures the real error against this bound at every BASELINE shape.
 KGE_DEV void tc_query_finish(const TcQueryArgs& T, const float* src, float th, int64_t q, int lane, int K) {
   __nv_bfloat16* o0 = T.A0 + (size_t)q * T.Kp;
   __nv_bfloat16* o1 = T.A1 + (size_t)q * T.Kp;

@@ -8,7 +8,7 @@
 // butterfly (4,2,1) is done as a reduce-scatter so that each lane finishes a different pair —
 // hence bit-identical to kge_score_fwd / the gather sweep / the CPU oracle.
 //
-// Data movement (B200): operand tiles are staged in shared memory by 2-D TMA tensor-map loads
+// Data movement: operand tiles are staged in shared memory by 2-D TMA tensor-map loads
 // (cp.async.bulk.tensor.2d, completion on an mbarrier; UTMALDG.2D in SASS), double buffered;
 // out-of-range rows / columns arrive zero-filled.  A tile is stored OCTET-MAJOR: one {32 columns
 // x rows} box per octet of the embedding axis lands as [octet][row][32 floats], so a group's 8

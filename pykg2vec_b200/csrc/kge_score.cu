@@ -36,8 +36,8 @@ score_fwd_kernel(ModelParams P, int grouping, const int64_t* __restrict__ h,
 
 // ---- TransE / TransM, large batches: persistent CTAs, rows staged in shared memory by cp.async --------
 // The register-cached kernel above holds a triple's three rows in registers (84 of its 115 registers at
-// d = 200), which caps it at 2 CTAs per SM that move in lock step through ids -> rows -> compute: measured
-// 4.2 TB/s of DRAM traffic (0.64 of the measured copy peak, profiles/r2_score_ch_sweep.jsonl).  Here a
+// d = 200), which caps it at 2 CTAs per SM that move in lock step through ids -> rows -> compute, so the
+// row loads of a CTA are never in flight while it computes.  Here a
 // CTA is persistent and software-pipelined: lane l of a group copies ITS chunks (l, l+8, ...) of the
 // three rows of the NEXT triple into a shared-memory stage with 16-byte cp.async (LDGSTS: no registers
 // are tied up, nothing waits), the ids of the triple after that are already in registers, and the current

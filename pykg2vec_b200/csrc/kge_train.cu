@@ -45,8 +45,7 @@ train_hinge_kernel(ModelParams P, GradTablesT GT, const int64_t* __restrict__ ph
     prefetch_triple_rows(Rn, P.d, P.dr, lane);
     // CHSEL = 0: the looped (not register-cached, not unrolled-by-width) forms of the score / gradient
     // functions.  A training batch is a few hundred groups — pure latency —, and the cached forms made this
-    // kernel 12,760 instructions (204 KB): ncu showed it stalled on INSTRUCTION FETCH (no_instruction 8.9 per
-    // issue, 30 us for 512 pairs; profiles/r2_ncu_step_v2_summary.txt).  Same arithmetic order, same bits.
+    // kernel 12,760 instructions (204 KB) and stalled it on instruction fetch.  Same arithmetic order, same bits.
     const float sp = score_group<MODEL, VEC, KGE_GROUP_TAIL, 0>(Rp, P, lane, scratch);
     const float sn = score_group<MODEL, VEC, KGE_GROUP_TAIL, 0>(Rn, P, lane, scratch);
     v = fmaxf(fsub(fadd(sp, margin), sn), 0.f);  // Criterion.pairwise_hinge, criterion.py:26-29
@@ -601,8 +600,8 @@ extern "C" int kge_train_pairwise_selfadv(const kge_model_t* m, float* const* gr
   }
   const int sf = (int)group_scratch_floats_bwd(m);
   // a warp per positive while each of its 4 groups has at most one negative; beyond that the whole CTA shares a
-  // positive (measured, profiles/r2_selfadv_fusion.jsonl: at neg_rate 16 the warp form — 4 triples in sequence per
-  // group, twice — is 14-37 % SLOWER than the five-launch path; the CTA form is at parity or ahead up to 256)
+  // positive (at neg_rate 16 the warp form runs 4 triples in sequence per group, twice, while the CTA form spreads
+  // them over the CTA; profiles/selfadv_fusion_probe.py times both against the five-launch path)
   const bool cta_team = neg_rate > 4;
   const size_t smem = ((size_t)sf * kGroupsPerCta + (size_t)(cta_team ? 1 : kThreads / 32) * (size_t)neg_rate) * sizeof(float);
   if (smem > 200 * 1024) {

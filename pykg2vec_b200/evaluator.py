@@ -234,7 +234,7 @@ class Evaluator:
 
     # ---- TransH / TransD: relation-grouped evaluation ---------------------------------------------
     GROUP_MIN_QUERIES_PER_RELATION = 32
-    GROUPED_BY_DEFAULT = None    # None: decide by queries per distinct relation (measured: profiles/r1_grouped_eval_v1.jsonl)
+    GROUPED_BY_DEFAULT = None    # None: decide by queries per distinct relation (bench_grouped.py times both paths)
 
     def _use_relation_groups(self, rs):
         """TransH / TransD project the candidate rows with a relation-dependent vector, so their

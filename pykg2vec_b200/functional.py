@@ -15,7 +15,7 @@ def _require_cuda(*tensors):
     for t in tensors:
         if not t.is_cuda:
             raise _lib.KgeError(
-                "pykg2vec_b200 runs on CUDA (sm_100a) only: got a %s tensor. There is no CPU "
+                "pykg2vec_b200 runs on CUDA (sm_90a) only: got a %s tensor. There is no CPU "
                 "fallback — move the model and ids to a CUDA device." % t.device)
 
 

@@ -1,5 +1,6 @@
 """Shared by the drop-in tests: the reference's own CLI flow (scripts/pykg2vec_train.py:11-23) on a
-UMLS-shaped synthetic dataset, with or without the B200 classes patched into Importer."""
+UMLS-shaped synthetic dataset, with or without this package's classes patched into Importer.  The reference is
+the unmodified package build() installs under oracle/_ref/ (oracle/reference.py)."""
 import os
 import sys
 
@@ -8,6 +9,18 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 if ROOT not in sys.path:
     sys.path.insert(0, ROOT)
+
+
+def reference_available():
+    from baseline import ref_loader
+    from oracle import reference
+    return ref_loader.available(reference.REF_DIR)
+
+
+def load_reference():
+    from baseline import ref_loader
+    from oracle import reference
+    return ref_loader.load(reference.REF_DIR)
 
 
 def write_dataset(dirpath, name="syn", n_ent=135, n_rel=46, n_train=5216, n_valid=652, n_test=661, seed=0):
@@ -33,8 +46,7 @@ def write_dataset(dirpath, name="syn", n_ent=135, n_rel=46, n_train=5216, n_vali
 def b200_importer_class():
     """The maintainer's patch of INTEGRATION.md §2 as a subclass: the in-scope names resolve under
     pykg2vec_b200 instead of pykg2vec.models (pykg2vec/common.py:266-325) — two attributes change."""
-    from baseline import ref_loader
-    ref_loader.load()
+    load_reference()
     from pykg2vec.common import Importer
     import pykg2vec_b200
 
@@ -48,8 +60,7 @@ def b200_importer_class():
 
 def run_cli_flow(argv, importer_cls=None):
     """scripts/pykg2vec_train.py main(), verbatim, with the Importer class injectable.  Returns the trainer."""
-    from baseline import ref_loader
-    ref_loader.load()
+    load_reference()
     from pykg2vec.common import Importer, KGEArgParser
     from pykg2vec.data.kgcontroller import KnowledgeGraph
     from pykg2vec.utils.trainer import Trainer

@@ -1,7 +1,7 @@
 // tests/emu/cuda_runtime.h — TEST INFRASTRUCTURE: a host stand-in for <cuda_runtime.h>.
 //
 // There is no GPU in the build container.  To exercise the indexing / synchronisation logic of a
-// CUDA kernel before it ever reaches a B200, tests/emu/*.cpp compile the product's kernel headers
+// CUDA kernel before it ever reaches a GPU, tests/emu/*.cpp compile the product's kernel headers
 // (pykg2vec_b200/csrc/*.cuh) with g++ against THIS header (found first through -I tests/emu) and
 // run every CUDA thread of a block as a host thread: __syncthreads() is a barrier over the block,
 // __shfl_xor_sync an exchange among the lanes named by its mask, atomics are host atomics, and

@@ -20,7 +20,7 @@ namespace kge {
 void set_error(const char*, ...) {}
 int cuda_fail(cudaError_t, const char*) { return KGE_ECUDA; }
 void count_launch(int) {}
-int sm_count() { return 148; }
+int sm_count() { return 132; }
 int num_tables(int) { return 0; }
 }  // namespace kge
 

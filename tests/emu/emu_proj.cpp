@@ -16,7 +16,7 @@ namespace kge {  // host-side symbols kge_common.cuh declares (defined in kge_ab
 void set_error(const char*, ...) {}
 int cuda_fail(cudaError_t, const char*) { return KGE_ECUDA; }
 void count_launch(int) {}
-int sm_count() { return 148; }
+int sm_count() { return 132; }
 }  // namespace kge
 
 using namespace kge;

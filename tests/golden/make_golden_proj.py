@@ -146,7 +146,13 @@ def make_case(name, N, R, k, k1, b, seed):
         out["tr_gx_" + tag] = xd.grad.numpy().copy()
         out["tr_gE_" + tag] = E.grad.numpy().copy()
         out["tr_gb_" + tag] = bb.grad.numpy().copy()
+    # arrays over 1 MB (the d=100 fc.weight) go to golden/split/ in two row blocks (golden_util.load joins them)
+    big = {k: out.pop(k) for k in list(out) if getattr(out[k], "nbytes", 0) > (1 << 20)}
     np.savez_compressed(os.path.join(HERE, name + ".npz"), **out)
+    for k, v in big.items():
+        os.makedirs(os.path.join(HERE, "split"), exist_ok=True)
+        for part, rows in enumerate(np.array_split(v, 2)):
+            np.savez_compressed(os.path.join(HERE, "split", "%s.%d.npz" % (name, part)), **{k: rows})
     print("wrote", name, "loss", out["tr_loss"], "ranks[0]", out["ranks"][0], "preds", p_tail[0, :3].numpy())
 
 

@@ -28,7 +28,14 @@ def proj_state(g):
 
 
 def load(name):
-    return dict(np.load(os.path.join(GOLDEN_DIR, name + ".npz"), allow_pickle=False))
+    """A case; arrays too large for one fixture file are stored in row blocks under golden/split/
+    (<name>.<k>.npz, k = 0, 1, ...) and concatenated back here."""
+    g = dict(np.load(os.path.join(GOLDEN_DIR, name + ".npz"), allow_pickle=False))
+    for p in sorted(glob.glob(os.path.join(GOLDEN_DIR, "split", name + ".*.npz")),
+                    key=lambda p: int(p.rsplit(".", 2)[1])):
+        for k, v in np.load(p, allow_pickle=False).items():
+            g[k] = np.concatenate([g[k], v]) if k in g else v
+    return g
 
 
 def tables_of(g):

@@ -1,30 +1,29 @@
-"""Drop-in proof (SURVEY.md §8b, VERDICT r1 item 8): the REFERENCE's own Importer -> Trainer.build_model /
-train_model -> Evaluator -> infer_* flow (scripts/pykg2vec_train.py:11-23) runs unchanged with the B200
-classes patched into Importer.modelMap, and the checkpoint shipped with the reference loads through
-Trainer.load_model into the mirror.
+"""Drop-in proof (SURVEY.md §8b): the REFERENCE's own Importer -> Trainer.build_model / train_model -> Evaluator
+-> infer_* flow (scripts/pykg2vec_train.py:11-23) runs unchanged with this package's classes patched into
+Importer.modelMap, and a checkpoint written by the reference loads into them.
 
 BASELINE.json configs[0] (`pykg2vec-train -mn TransE -ds umls`, CPU plumbing) is served by the UNMODIFIED
 reference classes — the product has no CPU path by design (a CPU fallback would void every parity claim);
 test_config1_cli_flow_reference_cpu runs exactly that flow here on the UMLS-shaped synthetic dataset, and
-the -m gpu tests run the same flow through the B200 classes with `-device cuda`.
+the -m gpu test runs the same flow through this package's classes with `-device cuda`.  Both need the
+unmodified reference that build() installs under oracle/_ref/ (oracle/reference.py) and skip without it.
 
-Needs baseline/_ref (the unmodified reference, installed by baseline/install_ref.sh; travels to the GPU box)."""
-import os
-import sys
-
+The checkpoint test needs nothing outside the repository: a slice of the reference's
+examples/pretrained/TransE/model.vec.pt (FB15k, d=50, L1) and the reference's scores on it are stored in
+golden/pretrained_transe_fb15k_slice.npz (golden/make_golden.py)."""
 import numpy as np
 import pytest
 import torch
 
 import dropin_util as du
-from baseline import ref_loader
+import golden_util as gu
 
-needs_ref = pytest.mark.skipif(not ref_loader.available(), reason="baseline/_ref not installed (baseline/install_ref.sh)")
+needs_ref = pytest.mark.skipif(not du.reference_available(), reason="oracle/_ref not installed (no reference checkout at build())")
 CFG1 = ["-mn", "TransE", "-l", "2", "-ts", "1", "-tn", "50", "-npg", "1"]   # defaults otherwise: d=50, B=128, adam, L1, margin 0.8
 
 
 def _flow(tmp_path, monkeypatch, extra, importer_cls=None):
-    ref_loader.load()
+    du.load_reference()
     ds = du.write_dataset(str(tmp_path / "data"))
     monkeypatch.chdir(tmp_path)   # the reference creates ../dataset relative to the CWD (datasets.py:84-86)
     return du.run_cli_flow(CFG1 + ["-ds", "syn", "-dsp", ds] + extra, importer_cls)
@@ -45,9 +44,9 @@ def test_config1_cli_flow_reference_cpu(tmp_path, monkeypatch):
 @pytest.mark.parametrize("model,extra", [("TransE", []), ("DistMult", []), ("Complex", []),
                                          ("RotatE", ["-ngr", "4"]), ("TransH", []), ("Rescal", ["-k", "16"])])
 def test_reference_trainer_drives_b200_classes(tmp_path, monkeypatch, model, extra):
-    """the unmodified reference Trainer / Generator / Evaluator with the B200 model classes, -device cuda"""
+    """the unmodified reference Trainer / Generator / Evaluator with this package's model classes, -device cuda"""
     B200Importer = du.b200_importer_class()
-    ref_loader.load()
+    du.load_reference()
     ds = du.write_dataset(str(tmp_path / "data"))
     monkeypatch.chdir(tmp_path)
     argv = ["-mn", model, "-l", "2", "-ts", "1", "-tn", "50", "-npg", "1", "-ds", "syn", "-dsp", ds, "-device", "cuda"] + extra
@@ -62,7 +61,7 @@ def test_reference_trainer_drives_b200_classes(tmp_path, monkeypatch, model, ext
     # Trainer.infer_* (trainer.py:330-386) through the reference's Evaluator.test_*_rank
     assert len(tr.infer_tails(1, 10, topk=5)) == 5
     assert len(tr.infer_heads(10, 20, topk=5)) == 5
-    # the reference's ranks over the B200 forward == the batched rank kernel on the same weights
+    # the reference's ranks over this package's forward == the batched rank kernel on the same weights
     from pykg2vec_b200.evaluator import Evaluator as B200Evaluator
     ev = B200Evaluator(tr.model, tr.config)
     ev.full_test(epoch=0)
@@ -76,33 +75,23 @@ def test_reference_trainer_drives_b200_classes(tmp_path, monkeypatch, model, ext
     assert (got != want).mean() < 0.02, (got != want).mean()
 
 
-@needs_ref
 @pytest.mark.gpu
-def test_pretrained_checkpoint_loads_through_trainer_load_model(tmp_path, monkeypatch):
-    """examples/pretrained/TransE/model.vec.pt + config.npy (FB15k, d=50, L1) through the reference's
-    Trainer.load_model (trainer.py:399-419) with Importer resolving to the B200 TransE; scores equal the
-    reference class's on the same checkpoint."""
-    ref_loader.load()
-    import pykg2vec.utils.trainer as ref_trainer
-    from pykg2vec.models.pairwise import TransE as RefTransE
-    B200Importer = du.b200_importer_class()
-    monkeypatch.setattr(ref_trainer, "Importer", B200Importer)
-    ckpt = os.path.join(ref_loader.REF_DIR, "examples", "pretrained", "TransE")
-    tr = object.__new__(ref_trainer.Trainer)
-    import types
-    tr.config = types.SimpleNamespace(load_from_data=ckpt)
-    tr.model = None
-    tr.load_model(ckpt)
-    m = tr.model
-    assert type(m).__module__ == "pykg2vec_b200.pairwise" and m.ent_embeddings.weight.shape == (14951, 50)
+def test_pretrained_checkpoint_loads_like_the_reference(tmp_path):
+    """the checkpoint slice loads the way Trainer.load_model loads a checkpoint (`model.load_state_dict(
+    torch.load(path))`, pykg2vec/utils/trainer.py:399-419) and scores like the reference's own TransE."""
+    import pykg2vec_b200
+    g = gu.load("pretrained_transe_fb15k_slice")
+    n_ent, n_rel = g["table0"].shape[0], g["table1"].shape[0]
+    path = tmp_path / "model.vec.pt"
+    torch.save({"ent_embeddings.weight": torch.from_numpy(g["table0"]),
+                "rel_embeddings.weight": torch.from_numpy(g["table1"])}, str(path))
+    m = pykg2vec_b200.import_model("TransE")(tot_entity=n_ent, tot_relation=n_rel, hidden_size=int(g["kw_hidden_size"]),
+                                             l1_flag=bool(g["kw_l1_flag"]))
+    m.load_state_dict(torch.load(str(path), map_location="cpu"))
+    assert type(m).__module__ == "pykg2vec_b200.pairwise" and m.ent_embeddings.weight.shape == (n_ent, 50)
     m = m.cuda()
-    sd = torch.load(os.path.join(ckpt, "model.vec.pt"), map_location="cpu")
-    ref = RefTransE(tot_entity=14951, tot_relation=1345, hidden_size=50, l1_flag=True)
-    ref.load_state_dict(sd)
-    rng = np.random.RandomState(0)
-    h, r, t = (torch.from_numpy(rng.randint(n, size=4096)) for n in (14951, 1345, 14951))
     with torch.no_grad():
-        want = ref(h, r, t).numpy()
-        got = m(h.cuda(), r.cuda(), t.cuda()).cpu().numpy()
+        got = m(*(torch.from_numpy(g[k]).cuda() for k in ("h", "r", "t"))).cpu().numpy()
+    want = g["scores"]
     err = np.abs(got - want) / np.maximum(np.abs(want), 1e-2 * np.abs(want).max())
     assert err.max() < 1e-4, err.max()

@@ -6,7 +6,7 @@ __shfl_xor_sync, host atomics), through the same launch plans the C-ABI launcher
 pins before the GPU run: tiling and strides of the three GEMM uses, zero padding, split-K
 ranges, the half-warp count reduction, the filter correction and the BCE reduction — against the
 oracle (bit-exact where the arithmetic is canonical, tolerance where the summation order is free).
-The real kernels are checked on the B200 by tests/test_gpu_proj.py."""
+The real kernels are checked on the GPU by tests/test_gpu_proj.py."""
 import ctypes
 import os
 
@@ -16,6 +16,7 @@ import pytest
 import oracle
 
 import emu_build
+import golden_util as gu
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 
@@ -130,8 +131,8 @@ def test_emulated_bce(emu, B, N, sms):
 def test_emulated_conve_trunk(emu, name, Q):
     """gather + bn0 + conv + bn1 + relu kernel and the Linear GEMM, on the reference's own ConvE
     parameters: bit-exact vs the oracle, which is pinned on the reference's x (test_oracle_proj)."""
-    g = np.load(os.path.join(HERE, "golden", name + ".npz"))
-    state = {k[3:]: g[k] for k in g.files if k.startswith("sd_") and not k.startswith("sd_after_")}
+    g = gu.load(name)
+    state = gu.proj_state(g)
     k, k1, R = int(g["hidden_size"]), int(g["hidden_size_1"]), int(g["R"])
     keep = {f: np.ascontiguousarray(state[key], dtype=np.float32) for f, key in oracle.CONVE_KEYS.items()}
     p = oracle.KgeConve()

@@ -2,7 +2,7 @@
 device math behind kge_score_fwd and the gather sweep — run under the host emulation of
 tests/emu/ with the thread mapping of score_fwd_kernel, against the oracle, BIT FOR BIT, on the
 tables of every golden case (both groupings).  A regression net for the model math that needs no
-GPU; the compiled kernels themselves are checked on the B200 by tests/test_gpu_score_rank.py."""
+GPU; the compiled kernels themselves are checked on the GPU by tests/test_gpu_score_rank.py."""
 import ctypes
 
 import numpy as np
