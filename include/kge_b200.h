@@ -256,7 +256,8 @@ int kge_rank_1vsall(const kge_model_t* m, const kge_model_t* mq, int64_t row_lo,
 int kge_rank_last_sweep_ms(int direction, float* ms);
 int kge_rank_last_sweep_directions(void);
 /* Measurement aid: per-role clock64 timeline of CTA (0,0) of subsequent tc_sweep_kernel launches into the
- * device buffer buf[3][64] (NULL = off): role 0 TMA producer, 1 MMA issuer, 2 epilogue (see kge_rank.cu);
+ * device buffer buf[3][64] (NULL = off): role 0 TMA producer, 1 consumer warpgroup start, 2 epilogue begin / end
+ * per tile, slot 63 of role 2 the kernel entry (see kge_rank.cu);
  * behind them buf[192 + 2 i], buf[193 + 2 i] = %globaltimer (ns) at entry / exit of CTA i (linear id < 1024),
  * and buf[2*64 + 62] = clock64 at the exit of CTA 0: the buffer must hold 192 + 2048 int64. */
 int kge_debug_set_tc_trace(long long* buf);

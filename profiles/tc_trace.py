@@ -18,38 +18,35 @@ flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
 for rep in range(3):
     _lib.rank_1vsall(desc, *q, flags=FL)
 torch.cuda.synchronize()
-for mode in (os.environ.get("TC_TRACE_MODES", "0").split(",")):
-    os.environ["KGE_TC_EPI_MODE"] = mode
-    buf.zero_()
-    # untraced timing first (mean of 5, L2 flushed)
-    times = []
-    for rep in range(5):
-        flush.zero_(); torch.cuda.synchronize()
-        _lib.rank_1vsall(desc, *q, flags=FL | _lib.RANK_PROFILE)
-        torch.cuda.synchronize()
-        times.append(_lib.rank_last_sweep_ms(0))
-    _lib.lib().kge_debug_set_tc_trace(ctypes.c_void_p(buf.data_ptr()))
+buf.zero_()
+# untraced timing first (mean of 5, L2 flushed)
+times = []
+for rep in range(5):
     flush.zero_(); torch.cuda.synchronize()
     _lib.rank_1vsall(desc, *q, flags=FL | _lib.RANK_PROFILE)
     torch.cuda.synchronize()
-    ms = _lib.rank_last_sweep_ms(0)
-    _lib.lib().kge_debug_set_tc_trace(ctypes.c_void_p(0))
-    raw = buf.cpu().numpy()
-    t = raw[:192].reshape(3, 64)
-    spans = raw[192:].reshape(1024, 2)
-    spans = spans[spans[:, 0] != 0]
-    t0 = t[2, 63]
-    out = {"directions": _lib.rank_last_sweep_directions(), "epi_mode": mode, "kernel_ms_untraced": times, "kernel_ms_traced": ms}
-    # role 0: the TMA producer's stage waits; 1: consumer warpgroup start (warp 4); 2: epilogue begin / end per tile
-    for r, name in enumerate(("producer", "consumer_start", "epilogue")):
-        out[name] = [int(x - t0) for x in t[r, :62] if x != 0]
-    if len(spans):
-        s0 = spans[:, 0].min()
-        out["ctas"] = int(len(spans))
-        out["cta_start_ns_minmax"] = [0, int(spans[:, 0].max() - s0)]
-        out["cta_end_ns_minmax"] = [int(spans[:, 1].min() - s0), int(spans[:, 1].max() - s0)]
-        out["cta0_ns"] = int(spans[0, 1] - spans[0, 0]) if raw[192] else None
-        out["cta0_cycles"] = int(t[2, 62] - t0)
-        out["cta_duration_ns_percentiles_0_50_100"] = [int(x) for x in np.percentile(spans[:, 1] - spans[:, 0], [0, 50, 100])]
-    print(json.dumps(out))
-os.environ.pop("KGE_TC_EPI_MODE", None)
+    times.append(_lib.rank_last_sweep_ms(0))
+_lib.lib().kge_debug_set_tc_trace(ctypes.c_void_p(buf.data_ptr()))
+flush.zero_(); torch.cuda.synchronize()
+_lib.rank_1vsall(desc, *q, flags=FL | _lib.RANK_PROFILE)
+torch.cuda.synchronize()
+ms = _lib.rank_last_sweep_ms(0)
+_lib.lib().kge_debug_set_tc_trace(ctypes.c_void_p(0))
+raw = buf.cpu().numpy()
+t = raw[:192].reshape(3, 64)
+spans = raw[192:].reshape(1024, 2)
+spans = spans[spans[:, 0] != 0]
+t0 = t[2, 63]
+out = {"directions": _lib.rank_last_sweep_directions(), "kernel_ms_untraced": times, "kernel_ms_traced": ms}
+# role 0: the TMA producer's stage waits; 1: consumer warpgroup start (warp 4); 2: epilogue begin / end per tile
+for r, name in enumerate(("producer", "consumer_start", "epilogue")):
+    out[name] = [int(x - t0) for x in t[r, :62] if x != 0]
+if len(spans):
+    s0 = spans[:, 0].min()
+    out["ctas"] = int(len(spans))
+    out["cta_start_ns_minmax"] = [0, int(spans[:, 0].max() - s0)]
+    out["cta_end_ns_minmax"] = [int(spans[:, 1].min() - s0), int(spans[:, 1].max() - s0)]
+    out["cta0_ns"] = int(spans[0, 1] - spans[0, 0]) if raw[192] else None
+    out["cta0_cycles"] = int(t[2, 62] - t0)
+    out["cta_duration_ns_percentiles_0_50_100"] = [int(x) for x in np.percentile(spans[:, 1] - spans[:, 0], [0, 50, 100])]
+print(json.dumps(out))

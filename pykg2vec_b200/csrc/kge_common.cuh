@@ -33,18 +33,19 @@ int sm_count();
     if (_e != cudaSuccess) return ::kge::cuda_fail(_e, name);   \
   } while (0)
 
-// Largest vector width (in floats) usable for row loads of width `d` from tables
-// whose base pointers are all aligned accordingly.
-inline int pick_vec(const kge_model_t* m, int ntab, int d, int d2 = 0) {
+// Largest vector width (in floats) usable for row loads of width `d` from the tables
+// tabs[0 .. ntab) when their base pointers are all aligned accordingly.
+inline int pick_vec(const float* const* tabs, int ntab, int d, int d2 = 0) {
   int vec = 4;
   if (d % 4 != 0 || (d2 && d2 % 4 != 0)) vec = (d % 2 == 0 && (!d2 || d2 % 2 == 0)) ? 2 : 1;
   for (int k = 0; k < ntab; ++k) {
-    const uintptr_t a = (uintptr_t)m->tables[k];
+    const uintptr_t a = (uintptr_t)tabs[k];
     if (vec == 4 && (a & 15)) vec = 2;
     if (vec == 2 && (a & 7)) vec = 1;
   }
   return vec;
 }
+inline int pick_vec(const kge_model_t* m, int ntab, int d, int d2 = 0) { return pick_vec(m->tables, ntab, d, d2); }
 
 // ---- device side ---------------------------------------------------------------
 #define KGE_DEV __device__ __forceinline__
@@ -68,6 +69,18 @@ KGE_DEV float group_sum(float v) {
 // 1 / max(sqrt(sumsq), 1e-12)  — F.normalize(eps=1e-12) as a reciprocal multiply
 KGE_DEV float inv_norm_from_sumsq(float sumsq) {
   return __frcp_rn(fmaxf(__fsqrt_rn(sumsq), 1e-12f));
+}
+
+// Plain L2 distances are compared in the SUM domain (DESIGN.md §3 rule 7): sqrt_rn is monotone, so
+//   sqrt_rn(sum) < th   <=>   sum < T(th),   T(th) = min{x >= 0 : sqrt_rn(x) >= th},
+// and T is found exactly by walking a few ulps around th*th.  Saves the IEEE square root per
+// (query, candidate) pair without changing a single comparison result.
+KGE_DEV float sqrt_domain_threshold(float th) {
+  if (!(th > 0.f)) return 0.f;                       // sqrt(.) >= 0 is never below th (also th = NaN)
+  float x = fmul(th, th);                            // may round to +inf or to 0
+  while (__fsqrt_rn(x) >= th) x = __uint_as_float(__float_as_uint(x) - 1u);  // never reaches below +0: sqrt(0) < th
+  while (__fsqrt_rn(x) < th) x = __uint_as_float(__float_as_uint(x) + 1u);   // stops at +inf at the latest
+  return x;
 }
 
 // Canonical sin/cos: Cody-Waite by pi/2 (3 parts) + Cephes minimax polynomials,

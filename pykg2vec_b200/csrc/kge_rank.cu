@@ -59,43 +59,6 @@ sweep_gather_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t
   }
 }
 
-// One group per filter entry (q, e): subtract it from the filtered count when it
-// outranks the target.  Entries equal to the target or outside the row shard are skipped.
-template <int MODEL, int VEC, int GROUPING>
-__global__ void __launch_bounds__(kThreads)
-filter_correct_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t* __restrict__ qr,
-                      const int64_t* __restrict__ qt, const int64_t* __restrict__ tgt,
-                      const float* __restrict__ thr, const int64_t* __restrict__ ptr,
-                      const int64_t* __restrict__ idx, int64_t Q, int64_t nnz, int64_t row_lo,
-                      int64_t row_hi, int32_t* __restrict__ counts, int col, int scratch_floats) {
-  extern __shared__ float4 smem_f4[];
-  float* scratch = reinterpret_cast<float*>(smem_f4) + (size_t)(threadIdx.x >> 3) * scratch_floats;
-  const int lane = threadIdx.x & 7;
-  const int64_t k = (int64_t)blockIdx.x * kGroupsPerCta + (threadIdx.x >> 3);
-  // the true entry count lives in device memory (ptr[Q]); the host may pass a capacity
-  // (upper bound) as nnz so that the launch shape can stay fixed inside a CUDA graph
-  const int64_t nnz_true = min(nnz, __ldg(ptr + Q));
-  if (nnz_true <= 0) return;
-  const bool valid = k < nnz_true;
-  const int64_t kk = valid ? k : nnz_true - 1;
-  int64_t lo = 0, hi = Q;  // largest q with ptr[q] <= kk
-  while (hi - lo > 1) {
-    const int64_t mid = (lo + hi) >> 1;
-    if (__ldg(ptr + mid) <= kk) lo = mid; else hi = mid;
-  }
-  const int64_t q = lo;
-  const int64_t e = __ldg(idx + kk);
-  const bool skip = (e == __ldg(tgt + q)) || e < row_lo || e >= row_hi;
-  const int64_t el = skip ? 0 : e - row_lo;
-  TripleRows R;
-  if (GROUPING == KGE_GROUP_TAIL)
-    resolve_rows<MODEL>(R, P, P.qtab, P.tab, P.qtab, __ldg(qh + q), __ldg(qr + q), el);
-  else
-    resolve_rows<MODEL>(R, P, P.tab, P.qtab, P.qtab, el, __ldg(qr + q), __ldg(qt + q));
-  const float s = score_group<MODEL, VEC, GROUPING>(R, P, lane, scratch);
-  if (valid && !skip && lane == 0 && s < __ldg(thr + q)) atomicSub(counts + q * 4 + col + 1, 1);
-}
-
 // thresholds: the target's own score, evaluated on the query-side tables
 template <int MODEL, int VEC, int GROUPING>
 __global__ void __launch_bounds__(kThreads)
@@ -113,28 +76,31 @@ threshold_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t* _
   if (valid && lane == 0) thr[g] = s;
 }
 
-// Level 2 of the tensor-core sweep (kge_rank_tc.cu) + the filter pass, one kernel: both are exact
-// re-evaluations of listed (query, candidate) pairs with the canonical fp32 group function — the
-// arithmetic of kge_score_fwd and of the fp32 sweeps.
-//   items [0, total)            : pairs whose tensor-core accumulator fell inside the query's band:
-//                                 tc_counts[q] += 1 when the candidate really outranks the target
-//   items [total, total + nnz)  : filter entries (as filter_correct_kernel): filtered column -= 1
-// The fp32 tiled sweep enqueued behind this kernel then commits the direction (counts += tc_counts) or —
-// list overflow: ctrl[0] > cap or ctrl[1] — ranks it itself (sweep_tiled_kernel's entry, kge_rank_tiled.cu);
-// on overflow this kernel still applies the filter corrections.
+// Exact re-evaluation of listed (query, candidate) pairs with the canonical fp32 group function — the
+// arithmetic of kge_score_fwd and of the sweeps.  One 8-lane group per item:
+//   items [0, total)            : with a band list (ctrl != nullptr), the pairs whose tensor-core accumulator
+//                                 fell inside the query's band (kge_rank_tc.cu): tc_counts[q] += 1 when the
+//                                 candidate really outranks the target.  total = 0 when the list overflowed.
+//   items [total, total + nnz)  : the filter entries: the filtered column -= 1 when the entry outranks the
+//                                 target.  Entries equal to the target or outside the row shard are skipped.
+// With a band list the fp32 tiled sweep enqueued behind this kernel then commits the direction (counts +=
+// tc_counts) or — list overflow: ctrl[0] > cap or ctrl[1] — ranks it itself (sweep_tiled_body's entry,
+// kge_rank_tiled.cu); on overflow this kernel still applies the filter corrections.
 template <int MODEL, int VEC, int GROUPING>
 __global__ void __launch_bounds__(kThreads)
-band_resolve_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t* __restrict__ qr,
-                    const int64_t* __restrict__ qt, const float* __restrict__ thr,
-                    const unsigned long long* __restrict__ list, unsigned* __restrict__ ctrl, unsigned cap,
-                    int64_t Q, int32_t* __restrict__ tc_counts, const RankFilter F, int32_t* __restrict__ counts,
-                    int col, int scratch_floats) {
+resolve_pairs_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t* __restrict__ qr,
+                     const int64_t* __restrict__ qt, const float* __restrict__ thr,
+                     const unsigned long long* __restrict__ list, unsigned* __restrict__ ctrl, unsigned cap,
+                     int32_t* __restrict__ tc_counts, const RankFilter F, int64_t Q, int64_t row_lo, int64_t row_hi,
+                     int32_t* __restrict__ counts, int col, int scratch_floats) {
   extern __shared__ float4 smem_f4[];
   float* scratch = reinterpret_cast<float*>(smem_f4) + (size_t)(threadIdx.x >> 3) * scratch_floats;
   const int lane = threadIdx.x & 7;
-  const unsigned listed = *reinterpret_cast<volatile unsigned*>(&ctrl[0]);
-  const bool overflow = listed > cap || *reinterpret_cast<volatile unsigned*>(&ctrl[1]) != 0u;
+  const unsigned listed = ctrl ? *reinterpret_cast<volatile unsigned*>(&ctrl[0]) : 0u;
+  const bool overflow = listed > cap || (ctrl && *reinterpret_cast<volatile unsigned*>(&ctrl[1]) != 0u);
   const int64_t total = overflow ? 0 : (int64_t)listed;
+  // the true entry count lives in device memory (ptr[Q]); the host may pass a capacity
+  // (upper bound) as nnz so that the launch shape can stay fixed inside a CUDA graph
   const int64_t nnz_true = (F.ptr && F.idx && F.nnz > 0) ? min(F.nnz, __ldg(F.ptr + Q)) : 0;
   const int64_t items = total + nnz_true;
   for (int64_t k = (int64_t)blockIdx.x * kGroupsPerCta + (threadIdx.x >> 3); k < items;
@@ -156,8 +122,8 @@ band_resolve_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t
       }
       q = lo;
       const int64_t ge = __ldg(F.idx + kk);
-      skip = (ge == __ldg(F.tgt + q)) || ge < F.row_lo || ge >= F.row_hi;
-      e = skip ? 0 : ge - F.row_lo;
+      skip = (ge == __ldg(F.tgt + q)) || ge < row_lo || ge >= row_hi;
+      e = skip ? 0 : ge - row_lo;
     }
     TripleRows R;
     if (GROUPING == KGE_GROUP_TAIL)
@@ -181,44 +147,100 @@ SweepProfile* sweep_profile(int dir) {
 int check_model(const kge_model_t* m);
 int model_vec(const kge_model_t* m);
 
-int band_resolve(const kge_model_t* m, const kge_model_t* mq, int dir, const int64_t* qh, const int64_t* qr,
-                 const int64_t* qt, const float* thr, int64_t Q, const TcDirBuffers& B, const RankFilter& F,
-                 int32_t* counts, int col, cudaStream_t st) {
-  const ModelParams P = make_params(m, mq);
-  int vec = model_vec(m);
-  const int vq = model_vec(mq);
-  if (vq < vec) vec = vq;
-  const int sf = (int)group_scratch_floats(m);
-  const size_t smem = (size_t)sf * kGroupsPerCta * sizeof(float);
-  const unsigned grid = (unsigned)(2 * sm_count());
-#define SET_SMEM_BR(K)                                                                        \
-  if (smem > 40 * 1024)                                                                       \
-    KGE_CUDA_OK(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-#define CALL_BR(M, V)                                                                          \
-  do {                                                                                         \
-    if (dir == 0) { SET_SMEM_BR((band_resolve_kernel<M, V, KGE_GROUP_TAIL>));                  \
-      band_resolve_kernel<M, V, KGE_GROUP_TAIL><<<grid, kThreads, smem, st>>>(                 \
-          P, qh, qr, qt, thr, B.list, B.ctrl, B.cap, Q, B.tc_counts, F, counts, col, sf); }    \
-    else { SET_SMEM_BR((band_resolve_kernel<M, V, KGE_GROUP_HEAD>));                           \
-      band_resolve_kernel<M, V, KGE_GROUP_HEAD><<<grid, kThreads, smem, st>>>(                 \
-          P, qh, qr, qt, thr, B.list, B.ctrl, B.cap, Q, B.tc_counts, F, counts, col, sf); }    \
-  } while (0)
-  switch (m->model) {   // the models tc_supported() admits
-    case KGE_TRANSE: KGE_DISPATCH_VEC(KGE_TRANSE, vec, CALL_BR); break;
-    case KGE_DISTMULT: KGE_DISPATCH_VEC(KGE_DISTMULT, vec, CALL_BR); break;
-    case KGE_CP: KGE_DISPATCH_VEC(KGE_CP, vec, CALL_BR); break;
-    case KGE_COMPLEX: KGE_DISPATCH_VEC(KGE_COMPLEX, vec, CALL_BR); break;
-    case KGE_RESCAL: KGE_DISPATCH_VEC(KGE_RESCAL, vec, CALL_BR); break;
-    case KGE_ROTATE: KGE_DISPATCH_VEC(KGE_ROTATE, vec, CALL_BR); break;
-    default: set_error("band_resolve: model %d has no tensor-core sweep", (int)m->model); return KGE_ENOTSUP;
+static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+
+RankLayout rank_layout(const kge_model_t* m, int64_t Q) {
+  RankLayout L = {};
+  const size_t q = (size_t)Q;
+  L.thr[0] = 0;
+  L.thr[1] = q * sizeof(float);
+  size_t o = align_up(2 * q * sizeof(float), 256);
+  auto take = [&o](size_t bytes) { const size_t at = o; o += align_up(bytes, 256); return at; };
+  if (tiled_supported(m)) {
+    const size_t dp = (size_t)rank_dp(m), kq = (size_t)rank_kq(m->model);
+    for (int d = 0; d < 2; ++d) L.qvec[d] = take(q * kq * dp * sizeof(float));
+    for (int d = 0; d < 2; ++d) L.qscale[d] = take(q * sizeof(float));
+    // always reserved: the alignment of the tables is only known at call time
+    L.cand = take(kq * (size_t)m->num_ent * dp * sizeof(float));
+    if (tc_supported(m, (int64_t)1 << 20)) {   // model-level support (the row count is only known per call)
+      const size_t Kp = (size_t)tc_kp(m);
+      for (int d = 0; d < 2; ++d) {
+        for (int k = 0; k < 2; ++k) L.a[d][k] = take(q * Kp * 2);
+        L.tau[d] = take(q * 4 * sizeof(float));
+        L.tc_counts[d] = take(q * sizeof(int32_t));
+        L.ctrl[d] = take(256);
+        L.list[d] = take((size_t)tc_list_capacity(Q) * 8);
+      }
+      for (int k = 0; k < 2; ++k) L.b[k] = take((size_t)m->num_ent * Kp * 2);
+      L.cn = take((size_t)m->num_ent * sizeof(float));
+    }
   }
-#undef CALL_BR
-#undef SET_SMEM_BR
-  KGE_CHECK_LAUNCH("band_resolve_kernel");
+  L.total = o;
+  return L;
+}
+
+// launch parameters of the group-function kernels of this file
+struct GroupArgs { ModelParams P; int vec, sf; size_t smem; };
+static GroupArgs group_args(const RankCall& C) {
+  GroupArgs G;
+  G.P = make_params(C.m, C.mq);
+  G.vec = model_vec(C.m);
+  const int vq = model_vec(C.mq);
+  if (vq < G.vec) G.vec = vq;
+  G.sf = (int)group_scratch_floats(C.m);
+  G.smem = (size_t)G.sf * kGroupsPerCta * sizeof(float);
+  return G;
+}
+
+// thresholds of the gather path (the tiled paths compute them in prepare_queries)
+static int gather_thresholds(const RankCall& C, int dir, cudaStream_t st) {
+  const GroupArgs G = group_args(C);
+  decltype(&threshold_kernel<KGE_TRANSE, 4, KGE_GROUP_TAIL>) kernel;
+#define PICK(M, V) kernel = dir == 0 ? threshold_kernel<M, V, KGE_GROUP_TAIL> : threshold_kernel<M, V, KGE_GROUP_HEAD>
+  KGE_DISPATCH_MODEL_VEC(C.m->model, G.vec, PICK);
+#undef PICK
+  const int rc = smem_optin(kernel, G.smem);
+  if (rc) return rc;
+  kernel<<<(unsigned)((C.Q + kGroupsPerCta - 1) / kGroupsPerCta), kThreads, G.smem, st>>>(G.P, C.qh, C.qr, C.qt, C.Q,
+                                                                                          C.thr(dir), G.sf);
+  KGE_CHECK_LAUNCH("threshold_kernel");
   return KGE_OK;
 }
 
-static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
+static int gather_sweep(const RankCall& C, int dir, cudaStream_t st) {
+  const GroupArgs G = group_args(C);
+  decltype(&sweep_gather_kernel<KGE_TRANSE, 4, KGE_GROUP_TAIL>) kernel;
+#define PICK(M, V) kernel = dir == 0 ? sweep_gather_kernel<M, V, KGE_GROUP_TAIL> : sweep_gather_kernel<M, V, KGE_GROUP_HEAD>
+  KGE_DISPATCH_MODEL_VEC(C.m->model, G.vec, PICK);
+#undef PICK
+  const int rc = smem_optin(kernel, G.smem);
+  if (rc) return rc;
+  const dim3 grid((unsigned)((C.nc + kCandsPerCta - 1) / kCandsPerCta), (unsigned)C.Q);
+  kernel<<<grid, kThreads, G.smem, st>>>(G.P, C.qh, C.qr, C.qt, C.thr(dir), C.nc, C.counts, 2 * dir, G.sf);
+  KGE_CHECK_LAUNCH("sweep_gather_kernel");
+  return KGE_OK;
+}
+
+int resolve_pairs(const RankCall& C, int dir, cudaStream_t st) {
+  const RankFilter& F = C.filt[dir];
+  if (!C.use_tc && !(F.ptr && F.idx && F.nnz > 0)) return KGE_OK;
+  const GroupArgs G = group_args(C);
+  decltype(&resolve_pairs_kernel<KGE_TRANSE, 4, KGE_GROUP_TAIL>) kernel;
+#define PICK(M, V) kernel = dir == 0 ? resolve_pairs_kernel<M, V, KGE_GROUP_TAIL> : resolve_pairs_kernel<M, V, KGE_GROUP_HEAD>
+  KGE_DISPATCH_MODEL_VEC(C.m->model, G.vec, PICK);
+#undef PICK
+  const int rc = smem_optin(kernel, G.smem);
+  if (rc) return rc;
+  // the band list's length is only known on the device: grid-stride over two CTAs per SM;
+  // filters alone: one group per entry
+  const unsigned grid = C.use_tc ? (unsigned)(2 * sm_count()) : (unsigned)((F.nnz + kGroupsPerCta - 1) / kGroupsPerCta);
+  kernel<<<grid, kThreads, G.smem, st>>>(
+      G.P, C.qh, C.qr, C.qt, C.thr(dir), C.use_tc ? C.at<unsigned long long>(C.L.list[dir]) : nullptr,
+      C.use_tc ? C.at<unsigned>(C.L.ctrl[dir]) : nullptr, tc_list_capacity(C.Q),
+      C.use_tc ? C.at<int32_t>(C.L.tc_counts[dir]) : nullptr, F, C.Q, C.row_lo, C.row_hi, C.counts, 2 * dir, G.sf);
+  KGE_CHECK_LAUNCH("resolve_pairs_kernel");
+  return KGE_OK;
+}
 
 // Fork/join helper: the head-direction chain of a rank call runs on a side stream so that its
 // short preparation / filter kernels overlap the other direction's sweep (and fill the idle
@@ -246,15 +268,26 @@ static int side_stream(SideStream** out) {
   return KGE_OK;
 }
 
+static RankCall make_call(const kge_model_t* m, const kge_model_t* mq, int64_t row_lo, int64_t row_hi,
+                          const int64_t* qh, const int64_t* qr, const int64_t* qt, int64_t Q, int32_t* counts,
+                          void* workspace) {
+  RankCall C;
+  C.m = m; C.mq = mq; C.qh = qh; C.qr = qr; C.qt = qt;
+  C.Q = Q; C.nc = row_hi - row_lo; C.row_lo = row_lo; C.row_hi = row_hi;
+  C.filt[0] = C.filt[1] = RankFilter{nullptr, nullptr, 0, nullptr};
+  C.counts = counts; C.ws = reinterpret_cast<char*>(workspace);
+  C.L = rank_layout(m, Q);
+  C.use_tiled = C.use_tc = false;
+  return C;
+}
+
 }  // namespace kge
 
 using namespace kge;
 
 extern "C" int64_t kge_rank_workspace_bytes(const kge_model_t* m, int64_t Q) {
   if (!m || Q < 0) return 0;
-  size_t bytes = align_up((size_t)2 * (size_t)Q * sizeof(float), 256);
-  bytes += tiled_workspace_bytes(m, Q);
-  return (int64_t)bytes;
+  return (int64_t)rank_layout(m, Q).total;
 }
 
 extern "C" int kge_rank_1vsall(const kge_model_t* m, const kge_model_t* mq, int64_t row_lo,
@@ -279,132 +312,73 @@ extern "C" int kge_rank_1vsall(const kge_model_t* m, const kge_model_t* mq, int6
   }
   if (Q > 65535) { set_error("kge_rank_1vsall: Q=%lld > 65535, batch the queries", (long long)Q); return KGE_EINVAL; }
   if (workspace_bytes < kge_rank_workspace_bytes(m, Q)) { set_error("workspace too small"); return KGE_EWORKSPACE; }
-  if (!tgt_h) tgt_h = qh;
-  if (!tgt_t) tgt_t = qt;
-  const int64_t nc = row_hi - row_lo;
-  cudaStream_t st = (cudaStream_t)stream;
-  const ModelParams P = make_params(m, mq);
-  int vec = model_vec(m);
-  const int vq = model_vec(mq);
-  if (vq < vec) vec = vq;
-  const int sf = (int)group_scratch_floats(m);
-  const size_t smem = (size_t)sf * kGroupsPerCta * sizeof(float);
-  if (smem > 227 * 1024) { set_error("kge_rank_1vsall: embedding width too large for this model's scratch"); return KGE_ENOTSUP; }
-  float* thr_t = reinterpret_cast<float*>(workspace);
-  float* thr_h = thr_t + Q;
-  void* tiled_ws = reinterpret_cast<char*>(workspace) + align_up((size_t)2 * (size_t)Q * sizeof(float), 256);
-  const unsigned qgrid = (unsigned)((Q + kGroupsPerCta - 1) / kGroupsPerCta);
-  const dim3 sgrid((unsigned)((nc + kCandsPerCta - 1) / kCandsPerCta), (unsigned)Q);
-  const bool use_tiled = !(flags & KGE_RANK_FORCE_GATHER) && tiled_supported(m);
-  const bool use_tc = use_tiled && !(flags & KGE_RANK_NO_TC) && tc_supported(m, nc);
-  if (use_tiled) {
-    rc = tiled_prepare_candidates(m, nc, tiled_ws, Q, use_tc, st);
+  if (group_scratch_floats(m) * kGroupsPerCta * sizeof(float) > 227 * 1024) {
+    set_error("kge_rank_1vsall: embedding width too large for this model's scratch"); return KGE_ENOTSUP;
+  }
+  RankCall C = make_call(m, mq, row_lo, row_hi, qh, qr, qt, Q, counts, workspace);
+  C.filt[0] = RankFilter{filt_t_ptr, filt_t_idx, filt_t_nnz, tgt_t ? tgt_t : qt};
+  C.filt[1] = RankFilter{filt_h_ptr, filt_h_idx, filt_h_nnz, tgt_h ? tgt_h : qh};
+  C.use_tiled = !(flags & KGE_RANK_FORCE_GATHER) && tiled_supported(m);
+  C.use_tc = C.use_tiled && !(flags & KGE_RANK_NO_TC) && tc_supported(m, C.nc);
+  const cudaStream_t main_st = (cudaStream_t)stream;
+  if (C.use_tiled) {
+    rc = prepare_candidates(C, main_st);
     if (rc) return rc;
   }
-
   for (int d = 0; d < 2; ++d) {
     SweepProfile* sp = sweep_profile(d);
     sp->armed = (flags & KGE_RANK_PROFILE) != 0;
     sp->valid = false;
+    sp->ndirs = 1;
     if (sp->armed && !sp->beg) {
       KGE_CUDA_OK(cudaEventCreate(&sp->beg));
       KGE_CUDA_OK(cudaEventCreate(&sp->end));
     }
   }
-  const bool both = !(flags & (KGE_RANK_HEAD_ONLY | KGE_RANK_TAIL_ONLY));
+  const bool run[2] = {!(flags & KGE_RANK_HEAD_ONLY), !(flags & KGE_RANK_TAIL_ONLY)};
   // (CP / SimplE refill one shared candidate scratch per direction: their directions stay serial)
-  const bool dirs_independent = m->model != KGE_CP && m->model != KGE_SIMPLE && m->model != KGE_SIMPLE_IGNR;
-  const bool two_streams = both && use_tiled && dirs_independent && !(flags & KGE_RANK_SINGLE_STREAM);
+  const bool dirs_independent = m->model != KGE_CP && !is_simple(m->model);
+  const bool two_streams = run[0] && run[1] && C.use_tiled && dirs_independent && !(flags & KGE_RANK_SINGLE_STREAM);
+  // Both directions on the tensor cores: their query preparations run side by side, ONE launch sweeps both
+  // (grid.z = 2: same candidate operands; the launch / pipeline-ramp / drain overhead — a third of a 25 us
+  // sweep at the FB15k-237 shape — is paid once and the tile units of both directions balance over the SMs),
+  // then the two exact-resolution chains run side by side again.
+  const bool tc_both = C.use_tc && two_streams;
   SideStream* side = nullptr;
-  cudaStream_t main_st = st;
   if (two_streams) {
     rc = side_stream(&side);
     if (rc) return rc;
     KGE_CUDA_OK(cudaEventRecord(side->fork, main_st));          // after candidate preparation
     KGE_CUDA_OK(cudaStreamWaitEvent(side->stream, side->fork, 0));
   }
-  // Both directions on the tensor cores: their query preparations run side by side, ONE launch sweeps both
-  // (grid.z = 2: same candidate operands; the launch / pipeline-ramp / drain overhead — a third of a 25 us
-  // sweep at the FB15k-237 shape — is paid once and the tile units of both directions balance over the SMs),
-  // then the two exact-resolution chains run side by side again.
-  if (use_tc && two_streams) {
-    const RankFilter Ft = {filt_t_ptr, filt_t_idx, filt_t_nnz, tgt_t, row_lo, row_hi};
-    const RankFilter Fh = {filt_h_ptr, filt_h_idx, filt_h_nnz, tgt_h, row_lo, row_hi};
-    rc = tiled_sweep(m, mq, 0, qh, qr, qt, thr_t, Q, nc, counts, 0, tiled_ws, true, &Ft, nullptr, nullptr, main_st, kSweepPrep);
+  auto stream_of = [&](int dir) { return (two_streams && dir == 1) ? side->stream : main_st; };
+  auto resolve_and_sweep = [&](int dir) {
+    const int r = resolve_pairs(C, dir, stream_of(dir));
+    if (r) return r;
+    return C.use_tiled ? tiled_sweep(C, dir, stream_of(dir)) : gather_sweep(C, dir, stream_of(dir));
+  };
+  for (int dir = 0; dir < 2; ++dir) {
+    if (!run[dir]) continue;
+    rc = C.use_tiled ? prepare_queries(C, dir, stream_of(dir)) : gather_thresholds(C, dir, stream_of(dir));
     if (rc) return rc;
-    rc = tiled_sweep(m, mq, 1, qh, qr, qt, thr_h, Q, nc, counts, 2, tiled_ws, true, &Fh, nullptr, nullptr, side->stream, kSweepPrep);
+    if (tc_both) continue;
+    if (C.use_tc) {
+      rc = tc_sweep(C, dir, 1, nullptr, stream_of(dir));
+      if (rc) return rc;
+    }
+    rc = resolve_and_sweep(dir);
     if (rc) return rc;
+  }
+  if (tc_both) {
     KGE_CUDA_OK(cudaEventRecord(side->mid, side->stream));
     KGE_CUDA_OK(cudaStreamWaitEvent(main_st, side->mid, 0));
-    rc = tiled_sweep(m, mq, 0, qh, qr, qt, thr_t, Q, nc, counts, 0, tiled_ws, true, &Ft, nullptr, nullptr, main_st, kSweepTc, true);
+    rc = tc_sweep(C, 0, 2, nullptr, main_st);
     if (rc) return rc;
     KGE_CUDA_OK(cudaEventRecord(side->fork2, main_st));
     KGE_CUDA_OK(cudaStreamWaitEvent(side->stream, side->fork2, 0));
-    rc = tiled_sweep(m, mq, 0, qh, qr, qt, thr_t, Q, nc, counts, 0, tiled_ws, true, &Ft, nullptr, nullptr, main_st, kSweepPost);
-    if (rc) return rc;
-    rc = tiled_sweep(m, mq, 1, qh, qr, qt, thr_h, Q, nc, counts, 2, tiled_ws, true, &Fh, nullptr, nullptr, side->stream, kSweepPost);
-    if (rc) return rc;
-    KGE_CUDA_OK(cudaEventRecord(side->join, side->stream));
-    KGE_CUDA_OK(cudaStreamWaitEvent(main_st, side->join, 0));
-    return KGE_OK;
-  }
-  for (int dir = 0; dir < 2; ++dir) {
-    if (dir == 0 && (flags & KGE_RANK_HEAD_ONLY)) continue;
-    if (dir == 1 && (flags & KGE_RANK_TAIL_ONLY)) continue;
-    st = (two_streams && dir == 1) ? side->stream : main_st;
-    float* thr = dir == 0 ? thr_t : thr_h;
-    const int col = dir == 0 ? 0 : 2;
-    const int64_t* fptr = dir == 0 ? filt_t_ptr : filt_h_ptr;
-    const int64_t* fidx = dir == 0 ? filt_t_idx : filt_h_idx;
-    const int64_t nnz = dir == 0 ? filt_t_nnz : filt_h_nnz;
-    const int64_t* tgt = dir == 0 ? tgt_t : tgt_h;
-#define SET_SMEM(K)                                                                          \
-  if (smem > 40 * 1024)                                                                      \
-    KGE_CUDA_OK(cudaFuncSetAttribute(K, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-#define CALL_THR(M, V)                                                                         \
-  do {                                                                                         \
-    if (dir == 0) { SET_SMEM((threshold_kernel<M, V, KGE_GROUP_TAIL>));                        \
-      threshold_kernel<M, V, KGE_GROUP_TAIL><<<qgrid, kThreads, smem, st>>>(P, qh, qr, qt, Q, thr, sf); } \
-    else { SET_SMEM((threshold_kernel<M, V, KGE_GROUP_HEAD>));                                 \
-      threshold_kernel<M, V, KGE_GROUP_HEAD><<<qgrid, kThreads, smem, st>>>(P, qh, qr, qt, Q, thr, sf); } \
-  } while (0)
-    if (!use_tiled) {  // the tiled path computes the thresholds inside its query-prep kernel
-      KGE_DISPATCH_MODEL_VEC(m->model, vec, CALL_THR);
-      KGE_CHECK_LAUNCH("threshold_kernel");
-    }
-#undef CALL_THR
-
-    if (use_tiled) {
-      const RankFilter F = {fptr, fidx, nnz, tgt, row_lo, row_hi};
-      rc = tiled_sweep(m, mq, dir, qh, qr, qt, thr, Q, nc, counts, col, tiled_ws, use_tc, &F, nullptr, nullptr, st);
+    for (int dir = 0; dir < 2; ++dir) {
+      rc = resolve_and_sweep(dir);
       if (rc) return rc;
-    } else {
-#define CALL_SWEEP(M, V)                                                                       \
-  do {                                                                                         \
-    if (dir == 0) { SET_SMEM((sweep_gather_kernel<M, V, KGE_GROUP_TAIL>));                     \
-      sweep_gather_kernel<M, V, KGE_GROUP_TAIL><<<sgrid, kThreads, smem, st>>>(P, qh, qr, qt, thr, nc, counts, col, sf); } \
-    else { SET_SMEM((sweep_gather_kernel<M, V, KGE_GROUP_HEAD>));                              \
-      sweep_gather_kernel<M, V, KGE_GROUP_HEAD><<<sgrid, kThreads, smem, st>>>(P, qh, qr, qt, thr, nc, counts, col, sf); } \
-  } while (0)
-      KGE_DISPATCH_MODEL_VEC(m->model, vec, CALL_SWEEP);
-#undef CALL_SWEEP
-      KGE_CHECK_LAUNCH("sweep_gather_kernel");
-    }
-
-    if (fptr && fidx && nnz > 0 && !use_tc) {   // (the tensor-core path's resolve kernel applies the filters)
-      const unsigned fgrid = (unsigned)((nnz + kGroupsPerCta - 1) / kGroupsPerCta);
-#define CALL_FILT(M, V)                                                                        \
-  do {                                                                                         \
-    if (dir == 0) { SET_SMEM((filter_correct_kernel<M, V, KGE_GROUP_TAIL>));                   \
-      filter_correct_kernel<M, V, KGE_GROUP_TAIL><<<fgrid, kThreads, smem, st>>>(              \
-          P, qh, qr, qt, tgt, thr, fptr, fidx, Q, nnz, row_lo, row_hi, counts, col, sf); }     \
-    else { SET_SMEM((filter_correct_kernel<M, V, KGE_GROUP_HEAD>));                            \
-      filter_correct_kernel<M, V, KGE_GROUP_HEAD><<<fgrid, kThreads, smem, st>>>(              \
-          P, qh, qr, qt, tgt, thr, fptr, fidx, Q, nnz, row_lo, row_hi, counts, col, sf); }     \
-  } while (0)
-      KGE_DISPATCH_MODEL_VEC(m->model, vec, CALL_FILT);
-#undef CALL_FILT
-      KGE_CHECK_LAUNCH("filter_correct_kernel");
     }
   }
   if (two_streams) {
@@ -414,8 +388,8 @@ extern "C" int kge_rank_1vsall(const kge_model_t* m, const kge_model_t* mq, int6
   return KGE_OK;
 }
 
-// Test / measurement aid for the tensor-core level of one direction: raw accumulators and the two
-// per-query thresholds (see include/kge_b200.h).
+// Test / measurement aid for the tensor-core level of one direction: raw accumulators and the band
+// (see include/kge_b200.h).  Runs the stages of kge_rank_1vsall for that direction without filters.
 extern "C" int kge_rank_tc_probe(const kge_model_t* m, const kge_model_t* mq, int64_t row_lo, int64_t row_hi,
                                  const int64_t* qh, const int64_t* qr, const int64_t* qt, int64_t Q, int direction,
                                  float* dots, float* tau, int32_t* counts, void* workspace, int64_t workspace_bytes,
@@ -429,18 +403,22 @@ extern "C" int kge_rank_tc_probe(const kge_model_t* m, const kge_model_t* mq, in
       row_hi - row_lo > m->num_ent || (direction != 0 && direction != 1)) {
     set_error("kge_rank_tc_probe: bad arguments"); return KGE_EINVAL;
   }
-  const int64_t nc = row_hi - row_lo;
-  if (!tiled_supported(m) || !tc_supported(m, nc)) {
+  if (!tiled_supported(m) || !tc_supported(m, row_hi - row_lo)) {
     set_error("kge_rank_tc_probe: no tensor-core sweep for this model / table size"); return KGE_ENOTSUP;
   }
   if (workspace_bytes < kge_rank_workspace_bytes(m, Q)) { set_error("workspace too small"); return KGE_EWORKSPACE; }
-  cudaStream_t st = (cudaStream_t)stream;
-  float* thr = reinterpret_cast<float*>(workspace) + (direction == 0 ? 0 : Q);
-  void* tiled_ws = reinterpret_cast<char*>(workspace) + align_up((size_t)2 * (size_t)Q * sizeof(float), 256);
-  rc = tiled_prepare_candidates(m, nc, tiled_ws, Q, true, st);
-  if (rc) return rc;
-  return tiled_sweep(m, mq, direction, qh, qr, qt, thr, Q, nc, counts, direction == 0 ? 0 : 2, tiled_ws, true, nullptr,
-                     dots, tau, st);
+  const cudaStream_t st = (cudaStream_t)stream;
+  RankCall C = make_call(m, mq, row_lo, row_hi, qh, qr, qt, Q, counts, workspace);
+  C.use_tiled = C.use_tc = true;
+  if ((rc = prepare_candidates(C, st)) || (rc = prepare_queries(C, direction, st)) ||
+      (rc = tc_sweep(C, direction, 1, dots, st)))
+    return rc;
+  if (tau) {   // [Q][4] band coefficients, then the nc candidate norm bounds
+    KGE_CUDA_OK(cudaMemcpyAsync(tau, C.ws + C.L.tau[direction], (size_t)Q * 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    KGE_CUDA_OK(cudaMemcpyAsync(tau + (size_t)Q * 4, C.ws + C.L.cn, (size_t)C.nc * sizeof(float), cudaMemcpyDeviceToDevice, st));
+  }
+  if ((rc = resolve_pairs(C, direction, st))) return rc;
+  return tiled_sweep(C, direction, st);
 }
 
 extern "C" int kge_rank_last_sweep_directions(void) {
@@ -459,8 +437,8 @@ extern "C" int kge_rank_last_sweep_ms(int direction, float* ms) {
 
 // Measurement aid: clock64 stamps of CTA (0,0) of the following tc_sweep_kernel launches are written to
 // buf[3 roles][64] (device memory; NULL switches it off).  Roles: 0 TMA producer (slot 0 start, then one
-// per acquired stage), 1 MMA issuer (start, queries resident, then per tile: accumulator free, per
-// k-block: stage full), 2 epilogue warp (start, per tile: accumulator ready, tile done; slot 63: kernel entry).
+// per acquired stage), 1 consumer warpgroup start (warp 4), 2 epilogue begin / end per tile (warp 4);
+// slot 63 of role 2: kernel entry, slot 62: cycles at the exit of CTA 0.
 extern "C" int kge_debug_set_tc_trace(long long* buf) {
   tc_set_trace(buf);
   return KGE_OK;

@@ -1,66 +1,111 @@
 // kge_rank.cuh — interface between the rank driver (kge_rank.cu), the fp32 tiled sweep
-// (kge_rank_tiled.cu) and the tensor-core sweep (kge_rank_tc.cu).
+// (kge_rank_tiled.cu) and the tensor-core sweep (kge_rank_tc.cu): the workspace layout, the
+// arguments of one rank call and the stages the driver runs for each direction.
 #pragma once
 #include "kge_common.cuh"
 
 namespace kge {
+
+// ---- model-level geometry ---------------------------------------------------------------------------
+inline bool is_simple(int model) { return model == KGE_SIMPLE || model == KGE_SIMPLE_IGNR; }
+// embedding width padded to whole 4-element chunks: row length of query vectors and candidate scratch
+inline int rank_dp(const kge_model_t* m) { return ((m->dim + 3) / 4) * 4; }
+// arrays per query vector and per candidate row of the tiled sweeps (KQ == KC): 2 for the two-term models
+constexpr int rank_kq(int model) {
+  return (model == KGE_ROTATE || model == KGE_COMPLEX || model == KGE_SIMPLE || model == KGE_SIMPLE_IGNR) ? 2 : 1;
+}
 bool tiled_supported(const kge_model_t* m);
-size_t tiled_workspace_bytes(const kge_model_t* m, int64_t Q);
-// Once per rank call: candidate-side scratch (normalised / padded copies, and the bf16 split of the
-// tensor-core path when `use_tc`) shared by both directions.
-int tiled_prepare_candidates(const kge_model_t* m, int64_t nc, void* ws, int64_t Q, bool use_tc, cudaStream_t st);
-// dir 0: tail sweep (TAIL grouping), 1: head sweep (HEAD grouping).  Writes the query vectors
-// AND the thresholds thr[q] (the target's own score), then adds
-// #{e < nc : score(q, e) < thr[q]} to counts[q*4+col] and counts[q*4+col+1].
-// use_tc: level 1 on the tensor cores + exact resolution of the ambiguous pairs (kge_rank_tc.cu);
-// the fp32 sweep is still enqueued but returns at once unless the pair list overflowed.
-// tc_dbg (tests): optional [Q][nc] raw tensor-core accumulators; tc_tau_out: optional [Q][4] band
-// coefficients followed by the nc candidate norm bounds.
-struct RankFilter;
-// phases (bit mask; the driver splits a direction's chain so that ONE tensor-core launch can sweep both
-// directions): kSweepPrep = query vectors, thresholds (+ CP's per-direction candidate operands);
-// kSweepTc = the tensor-core launch (tc_both: of both directions — call it for dir 0 only);
-// kSweepPost = level 2 + the fp32 sweep (the whole sweep when !use_tc, else the flag-gated fallback).
-constexpr int kSweepPrep = 1, kSweepTc = 2, kSweepPost = 4, kSweepAll = 7;
-int tiled_sweep(const kge_model_t* m, const kge_model_t* mq, int dir, const int64_t* qh,
-                const int64_t* qr, const int64_t* qt, float* thr, int64_t Q, int64_t nc,
-                int32_t* counts, int col, void* ws, bool use_tc, const RankFilter* filter, float* tc_dbg,
-                float* tc_tau_out, cudaStream_t st, int phases = kSweepAll, bool tc_both = false);
+bool tc_supported(const kge_model_t* m, int64_t nc);
+// tensor-core operand kind: 0 dot, 1 squared distance (sum domain), 2 squared distance - margin
+inline int tc_kind(const kge_model_t* m) { return (m->model == KGE_TRANSE) ? 1 : (m->model == KGE_ROTATE ? 2 : 0); }
+// contraction length of the tensor-core operands: KQ arrays of dp (+ the three norm columns), padded to 16
+inline int tc_kp(const kge_model_t* m) {
+  const int K = rank_kq(m->model) * rank_dp(m) + (tc_kind(m) != 0 ? 3 : 0);
+  return (K + 15) / 16 * 16;
+}
+// ambiguous-pair list slots per direction
+inline unsigned tc_list_capacity(int64_t Q) {
+  int64_t cap = 512 * Q;
+  if (cap < 32768) cap = 32768;   // (every consumer warp reserves one block of 16 up front: <= one wave of CTAs x 8 x 16 slots)
+  if (cap > (1 << 24)) cap = 1 << 24;
+  return (unsigned)cap;
+}
+
+// ---- the workspace ----------------------------------------------------------------------------------
+// Byte offsets of every region of a rank call's workspace; kge_rank_workspace_bytes is `total`.  The two
+// directions never share a query-side buffer: they may run concurrently on two streams.  The fp32 tiled
+// sweep's regions exist for tiled_supported models, the tensor-core regions for the models tc_supported
+// admits at some table size.
+struct RankLayout {
+  size_t thr[2];               // [Q] thresholds: the target's own score
+  size_t qvec[2];              // [Q][KQ][dp] query vectors of the tiled sweep
+  size_t qscale[2];            // [Q] TransM scale theta[r]
+  size_t cand;                 // [KC][num_ent][dp] candidate scratch (normalised / padded / realigned rows)
+  size_t a[2][2];              // [dir][0: high, 1: low] bf16 query operands [Q][Kp]
+  size_t tau[2];               // [Q][4] band coefficients (centre, a, b, e) of tc_query_finish
+  size_t tc_counts[2];         // [Q] certain counts of level 1 (+ the resolved pairs of level 2)
+  size_t ctrl[2];              // [4] pair-list length, overflow (+ 2 unused words)
+  size_t list[2];              // [tc_list_capacity(Q)] (q << 32 | local candidate row)
+  size_t b[2];                 // [0: high, 1: low] bf16 candidate operands [num_ent][Kp]
+  size_t cn;                   // [num_ent] candidate norm bounds
+  size_t total;
+};
+RankLayout rank_layout(const kge_model_t* m, int64_t Q);
+
+// ---- one rank call ----------------------------------------------------------------------------------
+// A direction's CSR filter (global entity ids) and the targets it must not count.
+struct RankFilter { const int64_t* ptr; const int64_t* idx; int64_t nnz; const int64_t* tgt; };
+
+// dir 0: tail sweep (TAIL grouping, counts columns 0/1), dir 1: head sweep (HEAD grouping, columns 2/3).
+struct RankCall {
+  const kge_model_t* m;        // candidate-side tables, rows [row_lo, row_hi)
+  const kge_model_t* mq;       // query-side tables
+  const int64_t *qh, *qr, *qt;
+  int64_t Q, nc, row_lo, row_hi;
+  RankFilter filt[2];
+  int32_t* counts;
+  char* ws;
+  RankLayout L;
+  bool use_tiled, use_tc;
+  template <class T> T* at(size_t off) const { return reinterpret_cast<T*>(ws + off); }
+  float* thr(int dir) const { return at<float>(L.thr[dir]); }
+};
+
+// The stages, in the order kge_rank_1vsall enqueues them for a direction (all capture-safe: no host sync,
+// no allocation):
+//   prepare_candidates   once per call (tiled paths): candidate scratch and, with use_tc, the bf16 candidate
+//                        operands shared by both directions
+//   prepare_queries      thresholds thr[q], the tiled sweep's query vectors and, with use_tc, the tensor-core
+//                        query operands and band coefficients; CP's per-direction candidate operands first
+//   tc_sweep             level 1 of one direction, or of both (ndirs == 2, dir == 0) in one grid.z = 2 launch;
+//                        dots: optional [Q][nc] raw accumulators of direction `dir` (tests)
+//   resolve_pairs        exact fp32 re-evaluation of listed pairs: the filter corrections, and with use_tc the
+//                        ambiguous pairs of level 1 into tc_counts
+//   tiled_sweep          the fp32 sweep; with use_tc its entry commits tc_counts to counts instead, unless the
+//                        pair list overflowed
+int prepare_candidates(const RankCall& C, cudaStream_t st);
+int prepare_queries(const RankCall& C, int dir, cudaStream_t st);
+int tc_sweep(const RankCall& C, int dir, int ndirs, float* dots, cudaStream_t st);
+int resolve_pairs(const RankCall& C, int dir, cudaStream_t st);
+int tiled_sweep(const RankCall& C, int dir, cudaStream_t st);
+
+// Used by the preparation stages of kge_rank_tiled.cu.  src[k]: the fp32 candidate tables (row pitch m->dim);
+// scratch: optional fp32 copy [KC][nc][dp] for the fp32 fallback sweep, written by the same kernel.
+int tc_prepare_candidates(const RankCall& C, const float* const src[2], float* scratch, cudaStream_t st);
+struct TcQueryArgs;
+TcQueryArgs tc_query_args(const RankCall& C, int dir);
 
 // Measurement hook (KGE_RANK_PROFILE): CUDA events recorded immediately around the launch of a
 // direction's main sweep kernel (tensor-core or fp32) on the stream it is launched on.
 struct SweepProfile { cudaEvent_t beg = nullptr, end = nullptr; bool armed = false, valid = false; int ndirs = 1; };
 SweepProfile* sweep_profile(int dir);
-
-// ---- tensor-core sweep (kge_rank_tc.cu) -------------------------------------------------------------
-struct TcDirBuffers {
-  int32_t* tc_counts;          // [Q] certain counts of level 1 (+ the resolved pairs of level 2)
-  unsigned* ctrl;              // [0] pair-list length, [1] overflow ([2], [3] unused)
-  unsigned long long* list;    // (q << 32 | local candidate row)
-  unsigned cap;
-  const float* tau;            // [Q][4] band coefficients (centre, a, b, e) of tc_query_finish
-  const float* cn;             // [nc] candidate norm bounds
-};
 void tc_set_trace(long long* buf);
-bool tc_supported(const kge_model_t* m, int64_t nc);
-size_t tc_workspace_bytes(const kge_model_t* m, int64_t Q);
-// src[k]: the model's own fp32 candidate tables (row pitch m->dim); scratch: optional fp32 copy
-// [KC][nc][dp] for the fp32 fallback sweep (normalised for TransE), written by the same kernel
-int tc_prepare_candidates(const kge_model_t* m, const float* const src[2], int64_t nc, void* tcws, int64_t Q,
-                          float* scratch, cudaStream_t st);
-struct TcQueryArgs;
-TcQueryArgs tc_query_args(const kge_model_t* m, int dir, void* tcws, int64_t Q);
-// ndirs == 2 (dir == 0): both directions in one launch (same candidate operands, grid.z = 2)
-int tc_sweep(const kge_model_t* m, int dir, int ndirs, int64_t Q, int64_t nc, void* tcws, float* dbg, cudaStream_t st);
-void tc_dir_buffers(const kge_model_t* m, int dir, int64_t Q, void* tcws, TcDirBuffers* out);
-// Level 2 (kge_rank.cu): exact fp32 re-evaluation of the listed pairs into tc_counts.  The fp32 sweep
-// enqueued next either commits the direction (counts[q*4+col], counts[q*4+col+1] += tc_counts[q]) or, if the
-// list overflowed, ranks the whole direction itself.
-// The same kernel also applies the direction's filter corrections (the entries of the CSR filter that
-// outrank the target are subtracted from the filtered column) — they are exact re-evaluations of
-// listed pairs too —, so the tensor-core path needs no separate filter pass.
-struct RankFilter { const int64_t* ptr; const int64_t* idx; int64_t nnz; const int64_t* tgt; int64_t row_lo, row_hi; };
-int band_resolve(const kge_model_t* m, const kge_model_t* mq, int dir, const int64_t* qh, const int64_t* qr,
-                 const int64_t* qt, const float* thr, int64_t Q, const TcDirBuffers& B, const RankFilter& F,
-                 int32_t* counts, int col, cudaStream_t st);
+
+// A kernel launched with more dynamic shared memory than the default 48 KB must opt in first.
+template <class Kernel>
+int smem_optin(Kernel kernel, size_t smem) {
+  if (smem > 40 * 1024)
+    KGE_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  return KGE_OK;
+}
 }  // namespace kge

@@ -18,7 +18,7 @@
 //         otherwise      -> (q, c) is appended to a list
 //     tau_hi/lo = centre -+ E with E a PROVEN bound on |D_tc - D_exact| + |canonical fp32 score -
 //     exact score| (prep_query below; derivation in DESIGN.md §4b).
-//   level 2 (kge_rank.cu, band_resolve_kernel): the listed pairs — a handful per query — are
+//   level 2 (kge_rank.cu, resolve_pairs_kernel): the listed pairs — a handful per query — are
 //     re-evaluated with the canonical fp32 group function (the arithmetic of kge_score_fwd /
 //     the fp32 sweeps / the CPU oracle) and compared exactly.
 //
@@ -30,14 +30,12 @@
 // (pykg2vec/utils/evaluator.py:249-273,309-334) for models pairwise.py:56-93 (TransE, -l1 False),
 // :765-791 (RotatE), :829-865 (Rescal), pointwise.py:444-446 (DistMult), :163-188 (Complex),
 // :374-376 (CP).
-#include <cuda.h>
 #include <cuda_bf16.h>
-
-#include <cstdlib>
 
 #include "kge_models.cuh"
 #include "kge_rank.cuh"
 #include "kge_rank_tc.cuh"
+#include "kge_tma.cuh"
 
 namespace kge {
 
@@ -68,44 +66,11 @@ struct TcParams {
   uint32_t tile_bytes;     // one operand k-block tile: 128 rows x kTcBK x 2 bytes
   int tiles_per_cta, ntiles;
   long long* trace;        // optional timeline of CTA (0,0): [3 roles][64] clock64 stamps (kge_debug_set_tc_trace)
-  int epi_mode;            // measurement aid (KGE_TC_EPI_MODE): 0 normal, 1 MMA only, 2 count only (no band listing)
 };
 // a*: query operands of blockIdx.z == 0, c*: of blockIdx.z == 1, b*: candidate operands
 struct TcMaps { CUtensorMap a0, a1, b0, b1, c0, c1; };
 
-// ---- PTX wrappers ---------------------------------------------------------------------------------
-KGE_DEV uint32_t tc_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-KGE_DEV void tc_mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(tc_smem_u32(bar)), "r"(count) : "memory");
-}
-KGE_DEV void tc_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(tc_smem_u32(bar)), "r"(bytes) : "memory");
-}
-KGE_DEV void tc_mbar_arrive(uint64_t* bar) {
-  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(tc_smem_u32(bar)) : "memory");
-}
-// Bounded wait: a protocol bug must end in a trap (a loud launch failure), never in a hung GPU.
-KGE_DEV void tc_mbar_wait(uint64_t* bar, uint32_t parity) {
-  const uint32_t addr = tc_smem_u32(bar);
-  const long long t0 = clock64();
-  for (;;) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(addr), "r"(parity) : "memory");
-    if (ok) return;
-    if (clock64() - t0 > 4000000000LL) __trap();   // ~2 s at 1.98 GHz
-  }
-}
-KGE_DEV void tc_tma_load_2d(uint32_t dst_smem, const CUtensorMap* tm, int col, int row, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-      ::"r"(dst_smem), "l"(reinterpret_cast<uint64_t>(tm)), "r"(col), "r"(row), "r"(tc_smem_u32(bar))
-      : "memory");
-}
-
+// ---- wgmma ---------------------------------------------------------------------------------------
 // shared-memory matrix descriptor (sm_90 wgmma): K-major operand tile [rows][64 bf16] written by TMA with the
 // 128-byte swizzle.  start address >> 4 in bits [0,14); leading byte offset (unused for swizzled K-major,
 // canonical value 1) in [16,30); stride byte offset = 8 rows x 128 B = 1024 (>> 4) in [32,46); layout type
@@ -156,7 +121,7 @@ KGE_DEV void tc_wgmma(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t a
 // Pair-list slots are handed out per WARP in blocks (16 slots) reserved with one global atomic (a returning
 // atomic per ambiguous pair would stall the epilogue on its round trip): base/size = the warp's current block
 // in P.list, used = slots already written.  Unused slots of a block are filled with the sentinel ~0
-// (band_resolve_kernel skips them), so [0, ctrl[0]) is always fully defined.
+// (resolve_pairs_kernel skips them), so [0, ctrl[0]) is always fully defined.
 struct TcListState { unsigned base, used, size; };
 constexpr unsigned long long kTcListHole = ~0ull;
 constexpr unsigned kTcListBlock = 16;
@@ -207,7 +172,7 @@ KGE_DEV void tc_epilogue(const float (&acc)[64], const float (&nl)[32], const Tc
       }
     }
   }
-  if (P.epi_mode != 2 && __any_sync(0xffffffffu, amb != 0)) {
+  if (__any_sync(0xffffffffu, amb != 0)) {
     int incl = amb;
 #pragma unroll
     for (int off = 1; off < 32; off <<= 1) {
@@ -269,7 +234,7 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
   const int t0 = blockIdx.x * P.tiles_per_cta;
   const int ntl = min(P.tiles_per_cta, P.ntiles - t0);
   if (ntl <= 0) return;
-  const uint32_t raw = tc_smem_u32(tc_smem_raw);
+  const uint32_t raw = smem_u32(tc_smem_raw);
   const uint32_t base = (raw + 1023u) & ~1023u;                 // SWIZZLE_128B tiles need 1024-byte alignment
   unsigned char* const gbase = tc_smem_raw + (base - raw);
   uint64_t* const full = reinterpret_cast<uint64_t*>(gbase);    // control block: first 1024 bytes
@@ -298,7 +263,7 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
   }
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < P.nstages; ++s) { tc_mbar_init(&full[s], 1); tc_mbar_init(&empty[s], kTcConsumerWarps); }
+    for (int s = 0; s < P.nstages; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], kTcConsumerWarps); }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
@@ -314,24 +279,24 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
       for (int t = 0; t < ntl; ++t) {
         const int row = (t0 + t) * kTcBN;
         for (int kb = 0; kb < P.nkb; ++kb) {
-          tc_mbar_wait(&empty[stage], phase ^ 1u);
+          mbar_wait(&empty[stage], phase ^ 1u);
           TC_STAMP(0, ev++);
           // resident query k-blocks ride on the FIRST tile's stage barriers, k-block by k-block: the first wgmma
           // needs one k-block of each operand in shared memory, not the whole query block
           const bool with_a = P.a_resident && t == 0;
-          tc_mbar_expect_tx(&full[stage], ((P.a_resident && !with_a) ? 2u : 4u) * tb);
+          mbar_arrive_expect_tx(&full[stage], ((P.a_resident && !with_a) ? 2u : 4u) * tb);
           const uint32_t sb = st_base + (uint32_t)stage * st_bytes;
           const int col = kb * kTcBK;
           if (with_a) {
             const uint32_t dst = a_base + (uint32_t)kb * 2u * tb;
-            tc_tma_load_2d(dst, ma0, col, (int)q0, &full[stage]);
-            tc_tma_load_2d(dst + tb, ma1, col, (int)q0, &full[stage]);
+            tma_load_2d(dst, ma0, col, (int)q0, &full[stage]);
+            tma_load_2d(dst + tb, ma1, col, (int)q0, &full[stage]);
           }
-          tc_tma_load_2d(sb, &TM.b0, col, row, &full[stage]);
-          tc_tma_load_2d(sb + tb, &TM.b1, col, row, &full[stage]);
+          tma_load_2d(sb, &TM.b0, col, row, &full[stage]);
+          tma_load_2d(sb + tb, &TM.b1, col, row, &full[stage]);
           if (!P.a_resident) {
-            tc_tma_load_2d(sb + 2u * tb, ma0, col, (int)q0, &full[stage]);
-            tc_tma_load_2d(sb + 3u * tb, ma1, col, (int)q0, &full[stage]);
+            tma_load_2d(sb + 2u * tb, ma0, col, (int)q0, &full[stage]);
+            tma_load_2d(sb + 3u * tb, ma1, col, (int)q0, &full[stage]);
           }
           if (++stage == P.nstages) { stage = 0; phase ^= 1u; }
         }
@@ -377,7 +342,7 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
         }
       int prev = -1;
       for (int kb = 0; kb < P.nkb; ++kb) {
-        tc_mbar_wait(&full[stage], phase);
+        mbar_wait(&full[stage], phase);
         const uint32_t sb = st_base + (uint32_t)stage * st_bytes;
         const uint32_t a0 = (P.a_resident ? a_base + (uint32_t)kb * 2u * tb : sb + 2u * tb) + a_off;
         const uint64_t da0 = tc_smem_desc(a0), da1 = tc_smem_desc(a0 + tb);
@@ -393,15 +358,15 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
         }
         tc_wgmma_commit();
         tc_wgmma_wait<1>();   // the group of the previous k-block has retired: its stage may be refilled
-        if (prev >= 0) { __syncwarp(); if (lane == 0) tc_mbar_arrive(&empty[prev]); }
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
         prev = stage;
         if (++stage == P.nstages) { stage = 0; phase ^= 1u; }
       }
       tc_wgmma_wait<0>();
       __syncwarp();
-      if (lane == 0) tc_mbar_arrive(&empty[prev]);
+      if (lane == 0) mbar_arrive(&empty[prev]);
       if (stamper) TC_STAMP(2, ev++);
-      if (P.epi_mode != 1) tc_epilogue(acc, nl, Bq, qa, cbase, nvalid, P, V, L, lane, cnt);
+      tc_epilogue(acc, nl, Bq, qa, cbase, nvalid, P, V, L, lane, cnt);
       if (stamper) TC_STAMP(2, ev++);
     }
     tc_list_pad(L, P, V, lane);   // the unused slots of the warp's last block become holes
@@ -483,17 +448,6 @@ static long long* g_tc_trace = nullptr;   // device buffer [3][64] or null (meas
 void tc_set_trace(long long* buf) { g_tc_trace = buf; }
 
 // ---- host side ------------------------------------------------------------------------------------
-static inline size_t tc_align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-static int tc_dp(const kge_model_t* m) { return ((m->dim + 3) / 4) * 4; }
-static int tc_kq(int model) { return (model == KGE_ROTATE || model == KGE_COMPLEX) ? 2 : 1; }
-static int tc_kind(const kge_model_t* m) {
-  return (m->model == KGE_TRANSE) ? 1 : (m->model == KGE_ROTATE ? 2 : 0);
-}
-static int tc_kp(const kge_model_t* m) {
-  const int K = tc_kq(m->model) * tc_dp(m) + (tc_kind(m) != 0 ? 3 : 0);
-  return (K + 15) / 16 * 16;
-}
-
 bool tc_supported(const kge_model_t* m, int64_t nc) {
   if (nc < 1024) return false;                      // small tables: the fp32 sweep is launch-latency sized anyway
   if (nc >= ((int64_t)1 << 31)) return false;
@@ -504,145 +458,58 @@ bool tc_supported(const kge_model_t* m, int64_t nc) {
   }
 }
 
-unsigned tc_list_capacity(int64_t Q) {
-  int64_t cap = 512 * Q;
-  if (cap < 32768) cap = 32768;   // (every consumer warp reserves one block of 16 up front: <= one wave of CTAs x 8 x 16 slots)
-  if (cap > (1 << 24)) cap = 1 << 24;
-  return (unsigned)cap;
-}
-
-// workspace carve-up (after the fp32 tiled sweep's region)
-struct TcLayout {
-  size_t a[2][2], tau[2], cnt[2], ctrl[2], list[2], b[2], cn, total;
-};
-static TcLayout tc_layout(const kge_model_t* m, int64_t Q) {
-  TcLayout L;
-  const size_t Kp = (size_t)tc_kp(m);
-  size_t o = 0;
-  for (int d = 0; d < 2; ++d) {
-    for (int k = 0; k < 2; ++k) { L.a[d][k] = o; o += tc_align_up((size_t)Q * Kp * 2, 256); }
-    L.tau[d] = o; o += tc_align_up((size_t)Q * 4 * sizeof(float), 256);
-    L.cnt[d] = o; o += tc_align_up((size_t)Q * sizeof(int32_t), 256);
-    L.ctrl[d] = o; o += 256;
-    L.list[d] = o; o += tc_align_up((size_t)tc_list_capacity(Q) * 8, 256);
-  }
-  for (int k = 0; k < 2; ++k) { L.b[k] = o; o += tc_align_up((size_t)m->num_ent * Kp * 2, 256); }
-  L.cn = o; o += tc_align_up((size_t)m->num_ent * sizeof(float), 256);
-  L.total = o;
-  return L;
-}
-size_t tc_workspace_bytes(const kge_model_t* m, int64_t Q) {
-  if (!tc_supported(m, (int64_t)1 << 20)) return 0;   // model-level support (row count is only known per call)
-  return tc_layout(m, Q).total;
-}
-
-typedef CUresult (*TcEncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                               const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                               CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static TcEncodeFn tc_encode_fn() {
-  static TcEncodeFn fn = nullptr;
-  if (fn) return fn;
-  void* p = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess || !p)
-    return nullptr;
-  fn = reinterpret_cast<TcEncodeFn>(p);
-  return fn;
-}
-// bf16 matrix [rows][Kp] row-major; box = {64 columns (128 bytes), 128 rows}, 128-byte swizzle, zero fill
-static int tc_make_map(CUtensorMap* tm, const void* base, uint64_t rows, uint64_t Kp) {
-  TcEncodeFn fn = tc_encode_fn();
-  if (!fn) { set_error("cuTensorMapEncodeTiled is not available"); return KGE_ECUDA; }
-  const cuuint64_t gdim[2] = {Kp, rows};
-  const cuuint64_t gstride[1] = {Kp * 2};
-  const cuuint32_t box[2] = {(cuuint32_t)kTcBK, (cuuint32_t)kTcBN};
-  const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled (bf16) failed (%d)", (int)r); return KGE_ECUDA; }
-  return KGE_OK;
-}
-
 // Candidate operands from the model's own fp32 tables src[k] (row pitch m->dim): bf16 split (+ norm
 // columns, + the per-row norm bounds) and, when `scratch` is given, the fp32 copy the fp32 fallback sweep reads
 // (normalised for TransE, zero padded to dp) — all in one kernel.
-int tc_prepare_candidates(const kge_model_t* m, const float* const src[2], int64_t nc, void* tcws, int64_t Q,
-                          float* scratch, cudaStream_t st) {
-  const TcLayout L = tc_layout(m, Q);
-  char* w = reinterpret_cast<char*>(tcws);
-  float* cn = reinterpret_cast<float*>(w + L.cn);
-  const int KC = tc_kq(m->model), d = m->dim, dp = tc_dp(m), Kp = tc_kp(m), aug = tc_kind(m) != 0 ? 1 : 0;
-  int vc = (d % 4 == 0) ? 4 : (d % 2 == 0 ? 2 : 1);
-  for (int k = 0; k < KC; ++k) {
-    const uintptr_t a = (uintptr_t)src[k];
-    if (vc == 4 && (a & 15)) vc = 2;
-    if (vc == 2 && (a & 7)) vc = 1;
-  }
-  const float* c0 = src[0];
-  const float* c1 = KC == 2 ? src[1] : src[0];
-  float* s0 = scratch;
-  float* s1 = (scratch && KC == 2) ? scratch + (size_t)nc * dp : nullptr;
-  __nv_bfloat16* B0 = reinterpret_cast<__nv_bfloat16*>(w + L.b[0]);
-  __nv_bfloat16* B1 = reinterpret_cast<__nv_bfloat16*>(w + L.b[1]);
-  const unsigned grid = (unsigned)((nc + 31) / 32);
-  const bool normalise = m->model == KGE_TRANSE;
-#define TC_PREP(V, NRM) tc_prep_cand_kernel<V, NRM><<<grid, 256, 0, st>>>(c0, c1, (int64_t)d, nc, d, dp, KC, Kp, aug, B0, B1, cn, s0, s1)
-  if (normalise) { if (vc == 4) TC_PREP(4, true); else if (vc == 2) TC_PREP(2, true); else TC_PREP(1, true); }
-  else { if (vc == 4) TC_PREP(4, false); else if (vc == 2) TC_PREP(2, false); else TC_PREP(1, false); }
-#undef TC_PREP
+int tc_prepare_candidates(const RankCall& C, const float* const src[2], float* scratch, cudaStream_t st) {
+  const kge_model_t* m = C.m;
+  const int64_t nc = C.nc;
+  const int KC = rank_kq(m->model), d = m->dim, dp = rank_dp(m), Kp = tc_kp(m), aug = tc_kind(m) != 0 ? 1 : 0;
+  const int vc = pick_vec(src, KC, d);
+  const bool nrm = m->model == KGE_TRANSE;
+  auto kernel = vc == 4 ? (nrm ? tc_prep_cand_kernel<4, true> : tc_prep_cand_kernel<4, false>)
+              : vc == 2 ? (nrm ? tc_prep_cand_kernel<2, true> : tc_prep_cand_kernel<2, false>)
+                        : (nrm ? tc_prep_cand_kernel<1, true> : tc_prep_cand_kernel<1, false>);
+  kernel<<<(unsigned)((nc + 31) / 32), 256, 0, st>>>(
+      src[0], KC == 2 ? src[1] : src[0], (int64_t)d, nc, d, dp, KC, Kp, aug, C.at<__nv_bfloat16>(C.L.b[0]),
+      C.at<__nv_bfloat16>(C.L.b[1]), C.at<float>(C.L.cn), scratch, (scratch && KC == 2) ? scratch + (size_t)nc * dp : nullptr);
   KGE_CHECK_LAUNCH("tc_prep_cand_kernel");
   return KGE_OK;
 }
 
 // Where prep_query_kernel (kge_rank_tiled.cu) leaves the tensor-core operands of direction `dir`.
-TcQueryArgs tc_query_args(const kge_model_t* m, int dir, void* tcws, int64_t Q) {
-  const TcLayout L = tc_layout(m, Q);
-  char* w = reinterpret_cast<char*>(tcws);
+TcQueryArgs tc_query_args(const RankCall& C, int dir) {
   TcQueryArgs T;
-  T.A0 = reinterpret_cast<__nv_bfloat16*>(w + L.a[dir][0]);
-  T.A1 = reinterpret_cast<__nv_bfloat16*>(w + L.a[dir][1]);
-  T.tau = reinterpret_cast<float*>(w + L.tau[dir]);
-  T.tc_counts = reinterpret_cast<int32_t*>(w + L.cnt[dir]);
-  T.ctrl = reinterpret_cast<unsigned*>(w + L.ctrl[dir]);
-  T.Kp = tc_kp(m); T.kind = tc_kind(m);
+  T.A0 = C.at<__nv_bfloat16>(C.L.a[dir][0]);
+  T.A1 = C.at<__nv_bfloat16>(C.L.a[dir][1]);
+  T.tau = C.at<float>(C.L.tau[dir]);
+  T.tc_counts = C.at<int32_t>(C.L.tc_counts[dir]);
+  T.ctrl = C.at<unsigned>(C.L.ctrl[dir]);
+  T.Kp = tc_kp(C.m); T.kind = tc_kind(C.m);
   // head sweep of TransE: canonical distance is |c + q| with q = r^ - t^  ->  contract with -q
-  T.sign = (m->model == KGE_TRANSE && dir == 1) ? -1.0f : 1.0f;
-  T.margin = m->margin;
+  T.sign = (C.m->model == KGE_TRANSE && dir == 1) ? -1.0f : 1.0f;
+  T.margin = C.m->margin;
   return T;
-}
-
-// The buffers level 2 reads for direction `dir` (no launch).
-void tc_dir_buffers(const kge_model_t* m, int dir, int64_t Q, void* tcws, TcDirBuffers* out) {
-  const TcLayout L = tc_layout(m, Q);
-  char* w = reinterpret_cast<char*>(tcws);
-  const TcQueryArgs T = tc_query_args(m, dir, tcws, Q);
-  out->tc_counts = T.tc_counts; out->ctrl = T.ctrl;
-  out->list = reinterpret_cast<unsigned long long*>(w + L.list[dir]);
-  out->cap = tc_list_capacity(Q); out->tau = T.tau; out->cn = reinterpret_cast<const float*>(w + L.cn);
 }
 
 // Level 1 (the query operands and thresholds were written by prep_query_kernel): the tensor-core sweep of
 // direction `dir`, or — ndirs == 2, dir == 0 — of both directions in ONE launch (grid.z = 2).  On return (in
 // stream order) tc_counts[q] holds the certain counts and list/ctrl the ambiguous pairs of each direction swept.
-int tc_sweep(const kge_model_t* m, int dir, int ndirs, int64_t Q, int64_t nc, void* tcws, float* dbg, cudaStream_t st) {
-  const TcLayout L = tc_layout(m, Q);
-  char* w = reinterpret_cast<char*>(tcws);
-  const int Kp = tc_kp(m);
+int tc_sweep(const RankCall& C, int dir, int ndirs, float* dots, cudaStream_t st) {
+  const RankLayout& L = C.L;
+  const int64_t Q = C.Q, nc = C.nc;
+  const int Kp = tc_kp(C.m);
   if (ndirs < 1 || ndirs > 2 || (ndirs == 2 && dir != 0)) { set_error("tc_sweep: bad direction set"); return KGE_EINVAL; }
+  const int dz[2] = {dir, ndirs == 2 ? dir + 1 : dir};   // (an unused second set mirrors the first)
   TcParams P;
-  const __nv_bfloat16* A0[2] = {nullptr, nullptr};
-  const __nv_bfloat16* A1[2] = {nullptr, nullptr};
   for (int z = 0; z < 2; ++z) {
-    const int dz = z < ndirs ? dir + z : dir;   // (an unused second set mirrors the first)
-    const TcQueryArgs T = tc_query_args(m, dz, tcws, Q);
-    P.D[z].tau = T.tau; P.D[z].tc_counts = T.tc_counts; P.D[z].ctrl = T.ctrl;
-    P.D[z].list = reinterpret_cast<unsigned long long*>(w + L.list[dz]);
-    P.D[z].dbg = (z == 0) ? dbg : nullptr;
-    A0[z] = T.A0; A1[z] = T.A1;
+    P.D[z].tau = C.at<float>(L.tau[dz[z]]);
+    P.D[z].tc_counts = C.at<int32_t>(L.tc_counts[dz[z]]);
+    P.D[z].ctrl = C.at<unsigned>(L.ctrl[dz[z]]);
+    P.D[z].list = C.at<unsigned long long>(L.list[dz[z]]);
+    P.D[z].dbg = (z == 0) ? dots : nullptr;
   }
-  P.cn = reinterpret_cast<const float*>(w + L.cn); P.cap = tc_list_capacity(Q);
+  P.cn = C.at<float>(L.cn); P.cap = tc_list_capacity(Q);
   P.tile_bytes = (uint32_t)(kTcBN * kTcBK * 2);
   P.Q = Q; P.nc = nc; P.Kp = Kp; P.nkb = (Kp + kTcBK - 1) / kTcBK;
   P.a_resident = Kp <= kTcResidentMaxK ? 1 : 0;
@@ -662,18 +529,19 @@ int tc_sweep(const kge_model_t* m, int dir, int ndirs, int64_t Q, int64_t nc, vo
   P.tiles_per_cta = (P.ntiles + splits - 1) / splits;
   splits = (P.ntiles + P.tiles_per_cta - 1) / P.tiles_per_cta;
   P.trace = g_tc_trace;
-  P.epi_mode = 0;
-  if (const char* e = getenv("KGE_TC_EPI_MODE")) P.epi_mode = atoi(e);   // measurement aid: wrong counts unless 0
+  // bf16 matrices [rows][Kp]; box = {64 columns (128 bytes), 128 rows}, 128-byte swizzle
   TcMaps TM;
-  int rc = tc_make_map(&TM.a0, A0[0], (uint64_t)Q, (uint64_t)Kp); if (rc) return rc;
-  rc = tc_make_map(&TM.a1, A1[0], (uint64_t)Q, (uint64_t)Kp); if (rc) return rc;
-  rc = tc_make_map(&TM.c0, A0[1], (uint64_t)Q, (uint64_t)Kp); if (rc) return rc;
-  rc = tc_make_map(&TM.c1, A1[1], (uint64_t)Q, (uint64_t)Kp); if (rc) return rc;
-  rc = tc_make_map(&TM.b0, w + L.b[0], (uint64_t)nc, (uint64_t)Kp); if (rc) return rc;
-  rc = tc_make_map(&TM.b1, w + L.b[1], (uint64_t)nc, (uint64_t)Kp); if (rc) return rc;
+  CUtensorMap* const maps[6] = {&TM.a0, &TM.a1, &TM.c0, &TM.c1, &TM.b0, &TM.b1};
+  const size_t offs[6] = {L.a[dz[0]][0], L.a[dz[0]][1], L.a[dz[1]][0], L.a[dz[1]][1], L.b[0], L.b[1]};
+  for (int k = 0; k < 6; ++k) {
+    const int rc = make_tensor_map(maps[k], CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, C.ws + offs[k], (uint64_t)(k < 4 ? Q : nc),
+                                   (uint64_t)Kp, (uint64_t)Kp * 2, kTcBK, kTcBN, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+  }
   const size_t smem = 2048 + a_bytes + (size_t)nstages * st_bytes;
+  const int rc = smem_optin(tc_sweep_kernel, smem);
+  if (rc) return rc;
   SweepProfile* sp = sweep_profile(dir);
-  KGE_CUDA_OK(cudaFuncSetAttribute(tc_sweep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
   if (sp->armed) KGE_CUDA_OK(cudaEventRecord(sp->beg, st));
   tc_sweep_kernel<<<dim3((unsigned)splits, (unsigned)qblocks, (unsigned)ndirs), kTcThreads, smem, st>>>(P, TM);
   KGE_CHECK_LAUNCH("tc_sweep_kernel");

@@ -54,15 +54,6 @@ KGE_DEV void tc_store_tail(__nv_bfloat16* o0, __nv_bfloat16* o1, int K, int Kp, 
   }
 }
 
-// The L2 sum-domain threshold of the fp32 sweep (rule 7 of DESIGN.md §3): T(th) = min{x : sqrt_rn(x) >= th}
-KGE_DEV float tc_sqrt_domain_threshold(float th) {
-  if (!(th > 0.f)) return 0.f;
-  float x = fmul(th, th);
-  while (__fsqrt_rn(x) >= th) x = __uint_as_float(__float_as_uint(x) - 1u);
-  while (__fsqrt_rn(x) < th) x = __uint_as_float(__float_as_uint(x) + 1u);
-  return x;
-}
-
 // Called by the 8 lanes of a query's group once its fp32 query vectors src[0 .. K) (K = KQ * dp, zero
 // padded, visible to the whole group) and its threshold th (the target's own canonical score) exist:
 // writes the bf16 split of the vectors (sign -1 for the head sweep of the translational models, whose
@@ -114,7 +105,7 @@ KGE_DEV void tc_query_finish(const TcQueryArgs& T, const float* src, float th, i
     double ks = 0.5 * g2;                        // coefficient of smax in the half band
     double a0 = ldexp(1.0, -50) * ss;
     if (T.kind == 1) {                           // canonical: sum < T(th)
-      const double Tt = (double)tc_sqrt_domain_threshold(th);
+      const double Tt = (double)sqrt_domain_threshold(th);
       centre = 0.5 * (ss - Tt);
     } else {                                     // canonical: fsub(sum, margin) < th
       centre = 0.5 * (ss - (double)th - (double)T.margin);

@@ -22,11 +22,10 @@
 //
 // Bound: fp32 pipe (2-8 instructions per element pair), not HBM: a candidate row is read from
 // L2 once per query BLOCK instead of once per query.
-#include <cuda.h>  // CUtensorMap (driver types only; the encoder is fetched through the runtime)
-
 #include "kge_models.cuh"
 #include "kge_rank.cuh"
 #include "kge_rank_tc.cuh"
+#include "kge_tma.cuh"
 
 namespace kge {
 
@@ -65,33 +64,6 @@ struct TiledParams {
   const int32_t* tc_counts;
 };
 
-// ---- mbarrier / bulk-copy primitives ------------------------------------------------------
-KGE_DEV uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-KGE_DEV void mbar_init(uint64_t* bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-KGE_DEV void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-KGE_DEV void mbar_wait(uint64_t* bar, uint32_t parity) {
-  uint32_t ok;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-  } while (!ok);
-}
-// 2-D tensor-map tile load (TMA): box {DS columns, rows} at (col, row) of a row-major fp32 matrix;
-// out-of-bounds elements are zero-filled and still counted in the transaction bytes.
-KGE_DEV void tma_load_2d(void* dst_smem, const CUtensorMap* tm, int col, int row, uint64_t* bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
-      ::"r"(smem_u32(dst_smem)), "l"(reinterpret_cast<uint64_t>(tm)), "r"(col), "r"(row), "r"(smem_u32(bar))
-      : "memory");
-}
-
 // ---- per-element pair operations (canonical arithmetic) ---------------------------------------
 // Two-term models (DOT2, ROT) accumulate chunk-wise — the chunk's 4 first terms, then its 4
 // second terms (DESIGN.md §3 rule 6) — so the two operand halves are consumed one after the other
@@ -119,18 +91,6 @@ KGE_DEV void pair_op(float& acc, const float4* q, const float4* c) {
 #pragma unroll
     for (int e = 0; e < 4; ++e) { const float si = fsub(f4_get(q[1], e), f4_get(c[1], e)); acc = ffma(si, si, acc); }
   }
-}
-
-// Plain L2 distances are compared in the SUM domain: sqrt_rn is monotone, so
-//   sqrt_rn(sum) < th   <=>   sum < T(th),   T(th) = min{x >= 0 : sqrt_rn(x) >= th},
-// and T is found exactly by walking a few ulps around th*th.  Saves the IEEE square root per
-// (query, candidate) pair without changing a single comparison result.
-KGE_DEV float sqrt_domain_threshold(float th) {
-  if (!(th > 0.f)) return 0.f;                       // sqrt(.) >= 0 is never below th (also th = NaN)
-  float x = fmul(th, th);                            // may round to +inf or to 0
-  while (__fsqrt_rn(x) >= th) x = __uint_as_float(__float_as_uint(x) - 1u);  // never reaches below +0: sqrt(0) < th
-  while (__fsqrt_rn(x) < th) x = __uint_as_float(__float_as_uint(x) + 1u);   // stops at +inf at the latest
-  return x;
 }
 
 template <int OP, bool L1>
@@ -265,11 +225,11 @@ __device__ __forceinline__ void sweep_tiled_body(const TiledParams& P, const Til
     if (lane32 < noct) {
       unsigned char* cdst = cbase + (size_t)stage * c_stage_bytes + (size_t)lane32 * kCOct;
       const int col = slab * DS + 32 * lane32;
-      tma_load_2d(cdst, &TM.c0, col, tile * kCBLK, &bars[stage]);
-      if (KC == 2) tma_load_2d(cdst + (size_t)kCBLK * 128u, &TM.c1, col, tile * kCBLK, &bars[stage]);
+      tma_load_2d(smem_u32(cdst), &TM.c0, col, tile * kCBLK, &bars[stage]);
+      if (KC == 2) tma_load_2d(smem_u32(cdst + (size_t)kCBLK * 128u), &TM.c1, col, tile * kCBLK, &bars[stage]);
       if (load_q)
-        tma_load_2d(qbase + (size_t)(P.nslabs > 1 ? stage : 0) * q_stage_bytes + (size_t)lane32 * kQOct, &TM.q, col,
-                    (int)(q0 * KQ), &bars[stage]);
+        tma_load_2d(smem_u32(qbase + (size_t)(P.nslabs > 1 ? stage : 0) * q_stage_bytes + (size_t)lane32 * kQOct),
+                    &TM.q, col, (int)(q0 * KQ), &bars[stage]);
     }
   };
 
@@ -427,8 +387,7 @@ prep_query_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t* 
   // threshold = the target's own score in this direction's grouping (== kge_score_fwd)
   const float s_target = score_group<MODEL, VEC, DIR == 0 ? KGE_GROUP_TAIL : KGE_GROUP_HEAD>(R, P, lane, scratch);
   if (lane == 0) thr[q] = s_target;
-  constexpr int KQ = (MODEL == KGE_COMPLEX || MODEL == KGE_SIMPLE || MODEL == KGE_SIMPLE_IGNR)
-                         ? 2 : (MODEL == KGE_ROTATE ? 2 : 1);
+  constexpr int KQ = rank_kq(MODEL);
   float* out = qvec + (size_t)q * KQ * dp;
   auto st = [&](int k, int c, float4 v) { *reinterpret_cast<float4*>(out + (size_t)k * dp + 4 * c) = v; };
   const float4 zero = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -581,15 +540,10 @@ prep_cand_kernel(const float* __restrict__ table, int64_t nc, int d, int dp, flo
 
 int model_vec(const kge_model_t* m);
 
-static inline size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
-static int dp_of(const kge_model_t* m) { return ((m->dim + 3) / 4) * 4; }
-static bool is_simple(int model) { return model == KGE_SIMPLE || model == KGE_SIMPLE_IGNR; }
-static int max_kq(int model) { return (model == KGE_ROTATE || model == KGE_COMPLEX || is_simple(model)) ? 2 : 1; }
-static int num_cand_tables(int model) { return (model == KGE_ROTATE || model == KGE_COMPLEX || is_simple(model)) ? 2 : 1; }
 // candidate source tables of a sweep direction; returns true when a scratch copy is needed
 // (normalised rows for TransE/TransM, padding for d % 4 != 0, unaligned tables)
 static bool cand_sources(const kge_model_t* m, int dir, const float* src[2]) {
-  const int KC = num_cand_tables(m->model);
+  const int KC = rank_kq(m->model);
   src[0] = src[1] = nullptr;
   if (m->model == KGE_CP) src[0] = m->tables[dir == 0 ? 2 : 0];
   else if (is_simple(m->model)) {  // TAIL: (t1, h2) = (ent_tail, ent_head)[c]; HEAD: (h1, t2) = (ent_head, ent_tail)[c]
@@ -600,58 +554,29 @@ static bool cand_sources(const kge_model_t* m, int dir, const float* src[2]) {
   return scratch;
 }
 
-static int fill_cand_scratch(const kge_model_t* m, const float* const src[2], int KC, int64_t nc,
-                             float* cscratch, cudaStream_t st) {
-  const int d = m->dim, dp = dp_of(m);
+static int fill_cand_scratch(const RankCall& C, const float* const src[2], cudaStream_t st) {
+  const kge_model_t* m = C.m;
+  const int KC = rank_kq(m->model), d = m->dim, dp = rank_dp(m);
   const bool normalise = (m->model == KGE_TRANSE || m->model == KGE_TRANSM);
-  int vc = (d % 4 == 0) ? 4 : (d % 2 == 0 ? 2 : 1);
+  const int vc = pick_vec(src, KC, d);
+  auto kernel = vc == 4 ? (normalise ? prep_cand_kernel<4, true> : prep_cand_kernel<4, false>)
+              : vc == 2 ? (normalise ? prep_cand_kernel<2, true> : prep_cand_kernel<2, false>)
+                        : (normalise ? prep_cand_kernel<1, true> : prep_cand_kernel<1, false>);
+  if (m->model == KGE_HOLE) kernel = prep_cand_even_kernel;
   for (int k = 0; k < KC; ++k) {
-    const uintptr_t a = (uintptr_t)src[k];
-    if (vc == 4 && (a & 15)) vc = 2;
-    if (vc == 2 && (a & 7)) vc = 1;
-  }
-  const unsigned cgrid = (unsigned)((nc + 31) / 32);
-  for (int k = 0; k < KC; ++k) {
-    float* dst = cscratch + (size_t)k * (size_t)nc * dp;
-    if (m->model == KGE_HOLE) {
-      prep_cand_even_kernel<<<cgrid, 256, 0, st>>>(src[k], nc, d, dp, dst);
-    } else if (normalise) {
-      if (vc == 4) prep_cand_kernel<4, true><<<cgrid, 256, 0, st>>>(src[k], nc, d, dp, dst);
-      else if (vc == 2) prep_cand_kernel<2, true><<<cgrid, 256, 0, st>>>(src[k], nc, d, dp, dst);
-      else prep_cand_kernel<1, true><<<cgrid, 256, 0, st>>>(src[k], nc, d, dp, dst);
-    } else {
-      if (vc == 4) prep_cand_kernel<4, false><<<cgrid, 256, 0, st>>>(src[k], nc, d, dp, dst);
-      else if (vc == 2) prep_cand_kernel<2, false><<<cgrid, 256, 0, st>>>(src[k], nc, d, dp, dst);
-      else prep_cand_kernel<1, false><<<cgrid, 256, 0, st>>>(src[k], nc, d, dp, dst);
-    }
+    kernel<<<(unsigned)((C.nc + 31) / 32), 256, 0, st>>>(src[k], C.nc, d, dp, C.at<float>(C.L.cand) + (size_t)k * (size_t)C.nc * dp);
     KGE_CHECK_LAUNCH("prep_cand_kernel");
   }
   return KGE_OK;
 }
 
-static float* cand_scratch_ptr(const kge_model_t* m, void* ws, int64_t Q) {
-  char* w = reinterpret_cast<char*>(ws);
-  w += 2 * align_up((size_t)Q * max_kq(m->model) * dp_of(m) * sizeof(float), 256);
-  w += 2 * align_up((size_t)Q * sizeof(float), 256);
-  return reinterpret_cast<float*>(w);
-}
-static size_t cand_scratch_bytes(const kge_model_t* m) {
-  return align_up((size_t)num_cand_tables(m->model) * (size_t)m->num_ent * (size_t)dp_of(m) * sizeof(float), 256);
-}
-// the tensor-core path's region follows the candidate scratch
-static void* tc_ws_ptr(const kge_model_t* m, void* ws, int64_t Q) {
-  return reinterpret_cast<char*>(cand_scratch_ptr(m, ws, Q)) + cand_scratch_bytes(m);
-}
-
-int tiled_prepare_candidates(const kge_model_t* m, int64_t nc, void* ws, int64_t Q, bool use_tc, cudaStream_t st) {
-  if (m->model == KGE_CP || is_simple(m->model)) return KGE_OK;  // per direction, see tiled_sweep
+int prepare_candidates(const RankCall& C, cudaStream_t st) {
+  if (C.m->model == KGE_CP || is_simple(C.m->model)) return KGE_OK;  // per direction: prepare_queries / tiled_sweep
   const float* src[2];
-  const int KC = num_cand_tables(m->model);
-  float* cscratch = cand_scratch_ptr(m, ws, Q);
-  const bool scratch = cand_sources(m, 0, src);
-  if (use_tc)   // one kernel: bf16 split for the tensor cores + (if the fp32 sweep needs one) its scratch copy
-    return tc_prepare_candidates(m, src, nc, tc_ws_ptr(m, ws, Q), Q, scratch ? cscratch : nullptr, st);
-  if (scratch) return fill_cand_scratch(m, src, KC, nc, cscratch, st);
+  const bool scratch = cand_sources(C.m, 0, src);
+  if (C.use_tc)   // one kernel: bf16 split for the tensor cores + (if the fp32 sweep needs one) its scratch copy
+    return tc_prepare_candidates(C, src, scratch ? C.at<float>(C.L.cand) : nullptr, st);
+  if (scratch) return fill_cand_scratch(C, src, st);
   return KGE_OK;
 }
 
@@ -664,167 +589,136 @@ bool tiled_supported(const kge_model_t* m) {
   }
 }
 
-size_t tiled_workspace_bytes(const kge_model_t* m, int64_t Q) {
-  if (!tiled_supported(m)) return 0;
-  const size_t dp = (size_t)dp_of(m);
-  size_t bytes = 2 * align_up((size_t)Q * max_kq(m->model) * dp * sizeof(float), 256);  // qvec, one per direction
-  bytes += 2 * align_up((size_t)Q * sizeof(float), 256);                                  // qscale, one per direction
-  // candidate scratch (always reserved: alignment of the tables is only known at call time);
-  // CP sweeps the object table for tails and the subject table for heads -> one table at a time
-  bytes += cand_scratch_bytes(m);
-  bytes += tc_workspace_bytes(m, Q);
-  return bytes;
+int prepare_queries(const RankCall& C, int dir, cudaStream_t st) {
+  const kge_model_t* m = C.m;
+  // CP sweeps the object table for tails and the subject table for heads: its tensor-core candidate
+  // operands are per direction and come first
+  if (m->model == KGE_CP && C.use_tc) {
+    const float* src[2] = {nullptr, nullptr};
+    const bool scratch = cand_sources(m, dir, src);
+    const int rc = tc_prepare_candidates(C, src, scratch ? C.at<float>(C.L.cand) : nullptr, st);
+    if (rc) return rc;
+  }
+  // query vectors and thresholds from the query-side tables
+  const ModelParams PQ = make_params(C.mq, C.mq);
+  const int vq = model_vec(C.mq);
+  const int psf = (int)group_scratch_floats(C.mq);
+  const size_t psmem = (size_t)psf * 32 * sizeof(float);
+  TcQueryArgs TCQ;
+  TCQ.A0 = nullptr;
+  if (C.use_tc) TCQ = tc_query_args(C, dir);
+  decltype(&prep_query_kernel<KGE_TRANSE, 4, 0>) kernel;
+#define PICK(M, V) kernel = dir == 0 ? prep_query_kernel<M, V, 0> : prep_query_kernel<M, V, 1>
+  switch (m->model) {
+    case KGE_HOLE: KGE_DISPATCH_VEC(KGE_HOLE, vq, PICK); break;
+    case KGE_RESCAL: KGE_DISPATCH_VEC(KGE_RESCAL, vq, PICK); break;
+    case KGE_SIMPLE: KGE_DISPATCH_VEC(KGE_SIMPLE, vq, PICK); break;
+    case KGE_SIMPLE_IGNR: KGE_DISPATCH_VEC(KGE_SIMPLE_IGNR, vq, PICK); break;
+    case KGE_TRANSE: KGE_DISPATCH_VEC(KGE_TRANSE, vq, PICK); break;
+    case KGE_TRANSM: KGE_DISPATCH_VEC(KGE_TRANSM, vq, PICK); break;
+    case KGE_DISTMULT: KGE_DISPATCH_VEC(KGE_DISTMULT, vq, PICK); break;
+    case KGE_CP: KGE_DISPATCH_VEC(KGE_CP, vq, PICK); break;
+    case KGE_COMPLEX: KGE_DISPATCH_VEC(KGE_COMPLEX, vq, PICK); break;
+    default: KGE_DISPATCH_VEC(KGE_ROTATE, vq, PICK); break;
+  }
+#undef PICK
+  const int rc = smem_optin(kernel, psmem);
+  if (rc) return rc;
+  kernel<<<(unsigned)((C.Q + 31) / 32), 256, psmem, st>>>(PQ, C.qh, C.qr, C.qt, C.Q, rank_dp(m), C.at<float>(C.L.qvec[dir]),
+                                                           C.at<float>(C.L.qscale[dir]), C.thr(dir), psf, TCQ);
+  KGE_CHECK_LAUNCH("prep_query_kernel");
+  return KGE_OK;
 }
 
-// cuTensorMapEncodeTiled through the runtime's driver-entry-point lookup (no -lcuda link)
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
                                   const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-static EncodeTiledFn encode_fn() {
+int make_tensor_map(CUtensorMap* tm, CUtensorMapDataType dtype, const void* base, uint64_t rows, uint64_t cols,
+                    uint64_t pitch_bytes, uint32_t box_cols, uint32_t box_rows, CUtensorMapSwizzle swizzle) {
   static EncodeTiledFn fn = nullptr;
-  if (fn) return fn;
-  void* p = nullptr;
-  cudaDriverEntryPointQueryResult qres;
-  if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) != cudaSuccess ||
-      qres != cudaDriverEntryPointSuccess || !p)
-    return nullptr;
-  fn = reinterpret_cast<EncodeTiledFn>(p);
-  return fn;
-}
-
-// row-major fp32 matrix [rows, cols] with row pitch `pitch` floats; box {box_cols, box_rows}
-static int make_map(CUtensorMap* tm, const float* base, uint64_t rows, uint64_t cols, uint64_t pitch,
-                    uint32_t box_cols, uint32_t box_rows) {
-  EncodeTiledFn fn = encode_fn();
-  if (!fn) { set_error("cuTensorMapEncodeTiled is not available"); return KGE_ECUDA; }
+  if (!fn) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qres) == cudaSuccess &&
+        qres == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<EncodeTiledFn>(p);
+    if (!fn) { set_error("cuTensorMapEncodeTiled is not available"); return KGE_ECUDA; }
+  }
   const cuuint64_t gdim[2] = {cols, rows};
-  const cuuint64_t gstride[1] = {pitch * sizeof(float)};
+  const cuuint64_t gstride[1] = {pitch_bytes};
   const cuuint32_t box[2] = {box_cols, box_rows};
   const cuuint32_t estr[2] = {1, 1};
-  const CUresult r = fn(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(base), gdim, gstride, box, estr,
-                        CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                        CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUresult r = fn(tm, dtype, 2, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                        swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (%d)", (int)r); return KGE_ECUDA; }
   return KGE_OK;
 }
 
 template <int OP, bool L1>
-static int launch_sweep(const TiledParams& P, int QBLK, size_t smem, cudaStream_t st, int splits, int qblocks) {
-  constexpr int KQ = OpTraits<OP>::KQ, KC = OpTraits<OP>::KC;
+static int launch_sweep(const TiledParams& P, size_t smem, dim3 grid, SweepProfile* prof, cudaStream_t st) {
+  constexpr int KQ = OpTraits<OP>::KQ, KC = OpTraits<OP>::KC, QBLK = kGQ * OpTraits<OP>::TQ;
   TiledMaps TM;
-  // one box = one octet: 32 columns x all rows of the tile (columns >= dp / rows >= extent read as zeros)
-  int rc = make_map(&TM.q, P.qvec, (uint64_t)P.Q * KQ, (uint64_t)P.dp, (uint64_t)P.dp, 32u, (uint32_t)(QBLK * KQ));
+  // fp32 matrices; one box = one octet: 32 columns x all rows of the tile (columns >= dp / rows >= extent read as zeros)
+  auto map = [&](CUtensorMap* tm, const float* base, uint64_t rows, uint64_t pitch, uint32_t box_rows) {
+    return make_tensor_map(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rows, (uint64_t)P.dp, pitch * sizeof(float), 32u,
+                           box_rows, CU_TENSOR_MAP_SWIZZLE_NONE);
+  };
+  int rc = map(&TM.q, P.qvec, (uint64_t)P.Q * KQ, (uint64_t)P.dp, (uint32_t)(QBLK * KQ));
   if (rc) return rc;
-  rc = make_map(&TM.c0, P.cand[0], (uint64_t)P.nc, (uint64_t)P.dp, (uint64_t)P.cand_pitch, 32u, (uint32_t)kCBLK);
+  rc = map(&TM.c0, P.cand[0], (uint64_t)P.nc, (uint64_t)P.cand_pitch, (uint32_t)kCBLK);
   if (rc) return rc;
+  TM.c1 = TM.c0;
   if (KC == 2) {
-    rc = make_map(&TM.c1, P.cand[1], (uint64_t)P.nc, (uint64_t)P.dp, (uint64_t)P.cand_pitch, 32u, (uint32_t)kCBLK);
+    rc = map(&TM.c1, P.cand[1], (uint64_t)P.nc, (uint64_t)P.cand_pitch, (uint32_t)kCBLK);
     if (rc) return rc;
-  } else {
-    TM.c1 = TM.c0;
   }
-  if constexpr (OP == OP_DOT2) {
-    KGE_CUDA_OK(cudaFuncSetAttribute(sweep_tiled_kernel_2cta<OP, L1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    sweep_tiled_kernel_2cta<OP, L1><<<dim3((unsigned)splits, (unsigned)qblocks), kTThreads, smem, st>>>(P, TM);
-  } else {
-    KGE_CUDA_OK(cudaFuncSetAttribute(sweep_tiled_kernel<OP, L1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    sweep_tiled_kernel<OP, L1><<<dim3((unsigned)splits, (unsigned)qblocks), kTThreads, smem, st>>>(P, TM);
-  }
+  const auto kernel = [] {
+    if constexpr (OP == OP_DOT2) return sweep_tiled_kernel_2cta<OP, L1>;
+    else return sweep_tiled_kernel<OP, L1>;
+  }();
+  rc = smem_optin(kernel, smem);
+  if (rc) return rc;
+  if (prof) KGE_CUDA_OK(cudaEventRecord(prof->beg, st));
+  kernel<<<grid, kTThreads, smem, st>>>(P, TM);
   KGE_CHECK_LAUNCH("sweep_tiled_kernel");
-  (void)QBLK;
+  if (prof) { KGE_CUDA_OK(cudaEventRecord(prof->end, st)); prof->valid = true; }
   return KGE_OK;
 }
 
-int tiled_sweep(const kge_model_t* m, const kge_model_t* mq, int dir, const int64_t* qh,
-                const int64_t* qr, const int64_t* qt, float* thr, int64_t Q, int64_t nc,
-                int32_t* counts, int col, void* ws, bool use_tc, const RankFilter* filter, float* tc_dbg,
-                float* tc_tau_out, cudaStream_t st, int phases, bool tc_both) {
-  const int model = m->model;
-  const int d = m->dim, dp = dp_of(m);
+int tiled_sweep(const RankCall& C, int dir, cudaStream_t st) {
+  const kge_model_t* m = C.m;
+  const int model = m->model, dp = rank_dp(m), KQ = rank_kq(model), KC = KQ;
+  const int64_t Q = C.Q, nc = C.nc;
   const int op = (model == KGE_TRANSE || model == KGE_TRANSM) ? (dir == 0 ? OP_TRANS_T : OP_TRANS_H)
                : (model == KGE_DISTMULT || model == KGE_CP || model == KGE_HOLE || model == KGE_RESCAL) ? OP_DOT1
                : (model == KGE_COMPLEX || is_simple(model)) ? OP_DOT2 : OP_ROT;
-  const int KQ = (op == OP_DOT2 || op == OP_ROT) ? 2 : 1;
-  const int KC = num_cand_tables(model);
   const int TQ = 4;
   const int QBLK = kGQ * TQ;
-  // workspace carve-up: [qvec dir0][qvec dir1][qscale dir0][qscale dir1][candidate scratch]
-  // (the two directions may run concurrently on two streams, so they never share query buffers)
-  char* w = reinterpret_cast<char*>(ws);
-  const size_t qvec_bytes = align_up((size_t)Q * max_kq(model) * dp * sizeof(float), 256);
-  const size_t qs_bytes = align_up((size_t)Q * sizeof(float), 256);
-  float* qvec = reinterpret_cast<float*>(w + (size_t)dir * qvec_bytes);
-  float* qscale = reinterpret_cast<float*>(w + 2 * qvec_bytes + (size_t)dir * qs_bytes);
-  float* cscratch = cand_scratch_ptr(m, ws, Q);
 
-  if (phases & kSweepPrep) {
-  // 0. CP sweeps the object table for tails and the subject table for heads: its tensor-core candidate
-  // operands (and max |c|^2, which the query thresholds read) are per direction and come first
-  if (model == KGE_CP && use_tc) {
-    const float* src[2] = {nullptr, nullptr};
-    const bool scratch = cand_sources(m, dir, src);
-    int rc = tc_prepare_candidates(m, src, nc, tc_ws_ptr(m, ws, Q), Q, scratch ? cscratch : nullptr, st);
-    if (rc) return rc;
-  }
-
-  // 1. query vectors (query-side tables)
-  const ModelParams PQ = make_params(mq, mq);
-  const int vq = model_vec(mq);
-  const unsigned qgrid = (unsigned)((Q + 31) / 32);
-  const int psf = (int)group_scratch_floats(mq);
-  const size_t psmem = (size_t)psf * 32 * sizeof(float);
-  TcQueryArgs TCQ;
-  TCQ.A0 = nullptr;
-  if (use_tc) TCQ = tc_query_args(m, dir, tc_ws_ptr(m, ws, Q), Q);
-#define PREP(M, V)                                                                                   \
-  do {                                                                                               \
-    if (dir == 0) {                                                                                  \
-      if (psmem > 40 * 1024) KGE_CUDA_OK(cudaFuncSetAttribute(prep_query_kernel<M, V, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem)); \
-      prep_query_kernel<M, V, 0><<<qgrid, 256, psmem, st>>>(PQ, qh, qr, qt, Q, dp, qvec, qscale, thr, psf, TCQ); \
-    } else {                                                                                         \
-      if (psmem > 40 * 1024) KGE_CUDA_OK(cudaFuncSetAttribute(prep_query_kernel<M, V, 1>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem)); \
-      prep_query_kernel<M, V, 1><<<qgrid, 256, psmem, st>>>(PQ, qh, qr, qt, Q, dp, qvec, qscale, thr, psf, TCQ); \
-    }                                                                                                \
-  } while (0)
-  switch (model) {
-    case KGE_HOLE: KGE_DISPATCH_VEC(KGE_HOLE, vq, PREP); break;
-    case KGE_RESCAL: KGE_DISPATCH_VEC(KGE_RESCAL, vq, PREP); break;
-    case KGE_SIMPLE: KGE_DISPATCH_VEC(KGE_SIMPLE, vq, PREP); break;
-    case KGE_SIMPLE_IGNR: KGE_DISPATCH_VEC(KGE_SIMPLE_IGNR, vq, PREP); break;
-    case KGE_TRANSE: KGE_DISPATCH_VEC(KGE_TRANSE, vq, PREP); break;
-    case KGE_TRANSM: KGE_DISPATCH_VEC(KGE_TRANSM, vq, PREP); break;
-    case KGE_DISTMULT: KGE_DISPATCH_VEC(KGE_DISTMULT, vq, PREP); break;
-    case KGE_CP: KGE_DISPATCH_VEC(KGE_CP, vq, PREP); break;
-    case KGE_COMPLEX: KGE_DISPATCH_VEC(KGE_COMPLEX, vq, PREP); break;
-    default: KGE_DISPATCH_VEC(KGE_ROTATE, vq, PREP); break;
-  }
-#undef PREP
-  KGE_CHECK_LAUNCH("prep_query_kernel");
-  }   // kSweepPrep
-
-  // 2. candidate arrays (scratch copies were produced by tiled_prepare_candidates)
+  // candidate arrays: the model's tables, or the scratch copy (made by prepare_candidates, or filled here
+  // when the tables differ per direction)
   TiledParams P;
   {
     const float* src[2] = {nullptr, nullptr};
-    const bool scratch = cand_sources(m, dir, src);
-    if (scratch) {
+    float* cscratch = C.at<float>(C.L.cand);
+    if (cand_sources(m, dir, src)) {
       for (int k = 0; k < KC; ++k) P.cand[k] = cscratch + (size_t)k * (size_t)nc * dp;
       if (KC == 1) P.cand[1] = nullptr;
       P.cand_pitch = dp;
-      if (((model == KGE_CP && !use_tc) || is_simple(model)) && (phases & kSweepPost)) {  // tables differ per direction: (re)fill now
-        int rc = fill_cand_scratch(m, src, KC, nc, cscratch, st);
+      if ((model == KGE_CP && !C.use_tc) || is_simple(model)) {
+        const int rc = fill_cand_scratch(C, src, st);
         if (rc) return rc;
       }
     } else {
-      P.cand[0] = src[0]; P.cand[1] = src[1]; P.cand_pitch = d;
+      P.cand[0] = src[0]; P.cand[1] = src[1]; P.cand_pitch = m->dim;
     }
   }
 
-  // 3. shared-memory plan (DS = columns staged per iteration, a multiple of 32 = whole octets):
+  // shared-memory plan (DS = columns staged per iteration, a multiple of 32 = whole octets):
   // whole rows when two CTAs of them fit in one SM (228 KB minus 1 KB reserved per CTA), else
   // slabs of DS columns with the accumulators living across slabs
   const size_t budget = (228 * 1024) / 2 - 1024;
-  const size_t hdr = align_up(32 + 3 * (size_t)QBLK * 4, 128);
+  const size_t hdr = (32 + 3 * (size_t)QBLK * 4 + 127) / 128 * 128;
   auto bytes_for = [&](int DS, int qstages) {
     return hdr + ((size_t)QBLK * KQ * qstages + (size_t)kCBLK * KC * 2) * (size_t)DS * sizeof(float);
   };
@@ -837,30 +731,11 @@ int tiled_sweep(const kge_model_t* m, const kge_model_t* mq, int dir, const int6
     nslabs = (dp + DS - 1) / DS;
   }
   const size_t smem = bytes_for(DS, nslabs > 1 ? 2 : 1);
-  P.tc_ctrl = nullptr; P.tc_cap = 0; P.tc_counts = nullptr;
-  if (use_tc) {
-    // level 1 on the tensor cores, level 2 = exact fp32 resolution of the ambiguous pairs (+ the filter
-    // corrections, same kernel); the fp32 sweep below stays enqueued as the fallback and returns at once
-    // unless the pair list overflowed
-    TcDirBuffers B;
-    tc_dir_buffers(m, dir, Q, tc_ws_ptr(m, ws, Q), &B);
-    if (phases & kSweepTc) {
-      int rc = tc_sweep(m, dir, tc_both ? 2 : 1, Q, nc, tc_ws_ptr(m, ws, Q), tc_dbg, st);
-      if (rc) return rc;
-      if (tc_tau_out) {   // probe: [Q][4] band coefficients, then the nc candidate norm bounds
-        KGE_CUDA_OK(cudaMemcpyAsync(tc_tau_out, B.tau, (size_t)Q * 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        KGE_CUDA_OK(cudaMemcpyAsync(tc_tau_out + (size_t)Q * 4, B.cn, (size_t)nc * sizeof(float), cudaMemcpyDeviceToDevice, st));
-      }
-    }
-    if (phases & kSweepPost) {
-      RankFilter none = {nullptr, nullptr, 0, nullptr, 0, 0};
-      int rc = band_resolve(m, mq, dir, qh, qr, qt, thr, Q, B, filter ? *filter : none, counts, col, st);
-      if (rc) return rc;
-    }
-    P.tc_ctrl = B.ctrl; P.tc_cap = B.cap; P.tc_counts = B.tc_counts;
-  }
-  if (!(phases & kSweepPost)) return KGE_OK;
-  P.qvec = qvec; P.thr = thr; P.qscale = (model == KGE_TRANSM) ? qscale : nullptr;
+  P.tc_ctrl = C.use_tc ? C.at<unsigned>(C.L.ctrl[dir]) : nullptr;
+  P.tc_cap = C.use_tc ? tc_list_capacity(Q) : 0;
+  P.tc_counts = C.use_tc ? C.at<int32_t>(C.L.tc_counts[dir]) : nullptr;
+  P.qvec = C.at<float>(C.L.qvec[dir]); P.thr = C.thr(dir);
+  P.qscale = (model == KGE_TRANSM) ? C.at<float>(C.L.qscale[dir]) : nullptr;
   P.Q = Q; P.nc = nc; P.dp = dp; P.DS = DS; P.nslabs = nslabs;
   P.ntiles = (int)((nc + kCBLK - 1) / kCBLK);
   const int qblocks = (int)((Q + QBLK - 1) / QBLK);
@@ -870,25 +745,21 @@ int tiled_sweep(const kge_model_t* m, const kge_model_t* mq, int dir, const int6
   if (splits > P.ntiles) splits = P.ntiles;
   P.tiles_per_cta = (P.ntiles + splits - 1) / splits;
   splits = (P.ntiles + P.tiles_per_cta - 1) / P.tiles_per_cta;
-  P.counts = counts; P.col = col; P.l1 = m->l1_flag; P.margin = m->margin;
+  P.counts = C.counts; P.col = 2 * dir; P.l1 = m->l1_flag; P.margin = m->margin;
   P.fin = (model == KGE_HOLE) ? 1 : (is_simple(model) ? 2 : 0);
 
-  SweepProfile* sp = sweep_profile(dir);
-  const bool prof = sp->armed && !use_tc;   // with the tensor-core level the profiled kernel is tc_sweep_kernel
-  if (prof) KGE_CUDA_OK(cudaEventRecord(sp->beg, st));
-  int rc;
+  // with the tensor-core level the profiled kernel is tc_sweep_kernel
+  SweepProfile* prof = (sweep_profile(dir)->armed && !C.use_tc) ? sweep_profile(dir) : nullptr;
+  const dim3 grid((unsigned)splits, (unsigned)qblocks);
   switch (op) {
-    case OP_TRANS_T: rc = m->l1_flag ? launch_sweep<OP_TRANS_T, true>(P, QBLK, smem, st, splits, qblocks)
-                                     : launch_sweep<OP_TRANS_T, false>(P, QBLK, smem, st, splits, qblocks); break;
-    case OP_TRANS_H: rc = m->l1_flag ? launch_sweep<OP_TRANS_H, true>(P, QBLK, smem, st, splits, qblocks)
-                                     : launch_sweep<OP_TRANS_H, false>(P, QBLK, smem, st, splits, qblocks); break;
-    case OP_DOT1: rc = launch_sweep<OP_DOT1, false>(P, QBLK, smem, st, splits, qblocks); break;
-    case OP_DOT2: rc = launch_sweep<OP_DOT2, false>(P, QBLK, smem, st, splits, qblocks); break;
-    default: rc = launch_sweep<OP_ROT, false>(P, QBLK, smem, st, splits, qblocks); break;
+    case OP_TRANS_T: return m->l1_flag ? launch_sweep<OP_TRANS_T, true>(P, smem, grid, prof, st)
+                                       : launch_sweep<OP_TRANS_T, false>(P, smem, grid, prof, st);
+    case OP_TRANS_H: return m->l1_flag ? launch_sweep<OP_TRANS_H, true>(P, smem, grid, prof, st)
+                                       : launch_sweep<OP_TRANS_H, false>(P, smem, grid, prof, st);
+    case OP_DOT1: return launch_sweep<OP_DOT1, false>(P, smem, grid, prof, st);
+    case OP_DOT2: return launch_sweep<OP_DOT2, false>(P, smem, grid, prof, st);
+    default: return launch_sweep<OP_ROT, false>(P, smem, grid, prof, st);
   }
-  if (rc) return rc;
-  if (prof) { KGE_CUDA_OK(cudaEventRecord(sp->end, st)); sp->valid = true; }
-  return KGE_OK;
 }
 
 }  // namespace kge

@@ -203,6 +203,15 @@ def test_rank_direction_flags_and_empty_filters():
     big = torch.zeros(70000, dtype=torch.int64, device="cuda")
     with pytest.raises(L.KgeError):
         L.rank_1vsall(desc, big, big, big)
+    # profiled sweeps report how many directions their launch covered: the tensor-core sweep of a full call
+    # covers both, the fp32 sweep of one direction covers one, also right after a tensor-core call
+    om, _ = gpu.synthetic_case("distmult", 2000, 4, 64, seed=2)
+    desc = gpu.desc_from_oracle_model(om)
+    qh, qt = rng.randint(2000, size=Q), rng.randint(2000, size=Q)
+    L.rank_1vsall(desc, _cuda(qh), _cuda(qr), _cuda(qt), flags=L.RANK_PROFILE)
+    assert L.rank_last_sweep_directions() == 2
+    L.rank_1vsall(desc, _cuda(qh), _cuda(qr), _cuda(qt), flags=L.RANK_PROFILE | L.RANK_NO_TC | L.RANK_TAIL_ONLY)
+    assert L.rank_last_sweep_directions() == 1
 
 
 def test_evaluator_batches_large_query_sets():
