@@ -248,6 +248,43 @@ def selfadv(pos, neg, neg_rate, alpha):  # criterion.py:14-23
     return -n.mean() - p.mean()
 
 
+# ---- optimizer steps (torch.optim single-tensor update order, trainer.py:112-126) ----
+# fp64 restatements of one dense step of the optimizers the trainer builds, with torch's defaults for every
+# argument the trainer does not pass.  Arrays are float64 (numpy or torch); the hyperparameters are the float32
+# values the kernels receive (kge_optim_apply_dense / kge_optim_apply_rows), widened exactly, so the only
+# difference to the kernels is the rounding of each operation.  Each returns new arrays; the inputs are not changed.
+def _f64(x):
+    return x.double() if torch.is_tensor(x) else torch.from_numpy(x).double()
+
+
+def sgd_step(w, g, lr):
+    """torch.optim.SGD(lr): param.add_(grad, alpha=-lr).  Returns w'."""
+    return _f64(w) - float(lr) * _f64(g)
+
+
+def adagrad_step(w, g, state_sum, lr, eps=1e-10):
+    """torch.optim.Adagrad(lr) (lr_decay 0, initial_accumulator_value 0): state_sum.addcmul_(grad, grad);
+    std = state_sum.sqrt().add_(eps); param.addcdiv_(grad, std, value=-lr).  Returns (w', state_sum')."""
+    g = _f64(g)
+    s = _f64(state_sum) + g * g
+    return _f64(w) - float(lr) * (g / (torch.sqrt(s) + float(eps))), s
+
+
+def adam_step(w, g, exp_avg, exp_avg_sq, step, lr, beta1=0.9, beta2=0.999, eps=1e-8):
+    """torch.optim.Adam(lr) (no weight decay, no amsgrad) at step `step` >= 1:
+    exp_avg.lerp_(grad, 1 - beta1); exp_avg_sq.mul_(beta2).addcmul_(grad, grad, value=1 - beta2);
+    step_size = lr / (1 - beta1**step); denom = exp_avg_sq.sqrt() / sqrt(1 - beta2**step) + eps;
+    param.addcdiv_(exp_avg, denom, value=-step_size).  Returns (w', exp_avg', exp_avg_sq')."""
+    b1, b2 = float(beta1), float(beta2)
+    g = _f64(g)
+    m = _f64(exp_avg)
+    m = m + (g - m) * (1.0 - b1)
+    v = _f64(exp_avg_sq) * b2 + (1.0 - b2) * g * g
+    step_size = float(lr) / (1.0 - b1 ** step)
+    denom = torch.sqrt(v) / math.sqrt(1.0 - b2 ** step) + float(eps)
+    return _f64(w) - step_size * (m / denom), m, v
+
+
 # ---- evaluation (pykg2vec/utils/evaluator.py) ---------------------------------
 def _walk(order, target, known):
     """MetricCalculator.get_tail_rank / get_head_rank, evaluator.py:70-123:

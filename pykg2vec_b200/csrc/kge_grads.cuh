@@ -995,7 +995,7 @@ KGE_DEV void grad_group(const TripleRows& R, const GradRows& G, const ModelParam
     }
     if (clamp_h0) hdot = 0.f;
     if (clamp_t0) tdot = 0.f;
-    __syncwarp();
+    group_sync();   // this group's lanes only: callers branch per group (train_hinge_kernel: active pairs)
     for (int c = lane; c < nch; c += 8) {
       const float4 hv = ld_chunk<VEC>(R.h[0], c, d), tv = ld_chunk<VEC>(R.t[0], c, d);
       float4 gh, gtt;

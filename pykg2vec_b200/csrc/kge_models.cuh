@@ -485,7 +485,7 @@ KGE_DEV float score_group(const TripleRows& R, const ModelParams& P, int lane, f
       *reinterpret_cast<float4*>(hp + 4 * c) = ah;
       *reinterpret_cast<float4*>(tp + 4 * c) = at;
     }
-    __syncwarp();
+    group_sync();   // this group's lanes only: callers branch per group (train_hinge_kernel: active pairs)
     return trans_distance<GROUPING, CHSEL>(
         [&](int c) { return *reinterpret_cast<const float4*>(hp + 4 * c); },
         [&](int c) {

@@ -233,12 +233,15 @@ KGE_DEV float4 exch_zero_b128(float* addr) {
   return r;
 }
 
+// One element of an SGD / Adagrad step in torch's single-tensor order (param.add_(grad, alpha=-lr);
+// state_sum.addcmul_(grad, grad); param.addcdiv_(grad, state_sum.sqrt().add_(eps), value=-lr)).  The sparse
+// (apply_rows_kernel) and the dense (apply_dense_kernel) application both call it, so they give the same bits.
 template <int OPT>
 KGE_DEV float apply_elem(float wv, float gv, float* s, float lr, float eps) {
-  if (OPT == 0) return wv - lr * gv;
-  const float sv = *s + gv * gv;
+  if (OPT == 0) return ffma(-lr, gv, wv);
+  const float sv = ffma(gv, gv, *s);
   *s = sv;
-  return wv - lr * gv / (sqrtf(sv) + eps);
+  return fsub(wv, fmul(lr, __fdiv_rn(gv, fadd(__fsqrt_rn(sv), eps))));
 }
 
 template <int OPT>
@@ -376,12 +379,8 @@ apply_dense_kernel(float* __restrict__ w, float* __restrict__ g, float* __restri
     for (int e = 0; e < 4; ++e) {
       const float gg = f4_get(gv, e);
       float& ww = f4_at(wv, e);
-      if (OPT == 0) {
-        ww = ffma(-lr, gg, ww);
-      } else if (OPT == 1) {
-        float& ss = f4_at(a, e);
-        ss = ffma(gg, gg, ss);
-        ww = fsub(ww, fmul(lr, __fdiv_rn(gg, fadd(__fsqrt_rn(ss), eps))));
+      if (OPT <= 1) {
+        ww = apply_elem<OPT>(ww, gg, &f4_at(a, e), lr, eps);
       } else {
         float& m = f4_at(a, e);
         float& v = f4_at(b, e);
@@ -402,12 +401,12 @@ apply_dense_kernel(float* __restrict__ w, float* __restrict__ g, float* __restri
     const int64_t i = tail0 + threadIdx.x;
     const float gg = g[i];
     float ww = w[i];
-    if (OPT == 0) {
-      ww = ffma(-lr, gg, ww);
-    } else if (OPT == 1) {
-      const float ss = ffma(gg, gg, s1[i]);
-      s1[i] = ss;
-      if (gg != 0.f) ww = fsub(ww, fmul(lr, __fdiv_rn(gg, fadd(__fsqrt_rn(ss), eps))));
+    if (OPT <= 1) {
+      if (gg != 0.f) {   // SGD / Adagrad: nothing moves
+        float ss = OPT == 1 ? s1[i] : 0.f;
+        ww = apply_elem<OPT>(ww, gg, &ss, lr, eps);
+        if (OPT == 1) s1[i] = ss;
+      }
     } else {
       const float m = ffma(fsub(gg, s1[i]), 1.0f - b1, s1[i]);
       const float v = ffma(fmul(gg, gg), 1.0f - b2, fmul(s2[i], b2));

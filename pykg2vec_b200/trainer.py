@@ -11,8 +11,9 @@ Two execution modes for the same step semantics:
     as a few kernels with no autograd graph and no torch optimizer:
       pairwise hinge + SGD : kge_train_pairwise_hinge_sgd (2 kernels)
       sgd / adagrad        : score_fwd -> loss kernel -> score_bwd (+ reg) -> kge_optim_apply_rows
-                             (sparse: zero-gradient rows do not move under SGD/Adagrad, so the result
-                             equals the dense optimizers')
+                             (sparse: zero-gradient rows do not move under SGD/Adagrad, and the touched rows
+                             share kge_optim_apply_dense's per-element arithmetic, so the result equals the
+                             dense step bit for bit)
       adam (the CLI default, common.py:50): ... -> kge_optim_apply_dense per table — dense Adam moves
                              every row every step, so its exact form is one HBM-bound sweep per table
   * data-parallel (torch.distributed world > 1, tables replicated; SURVEY.md 8e row 3): config.dp_mode
