@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KGE_ABI_VERSION 5
+#define KGE_ABI_VERSION 6
 #define KGE_MAX_TABLES 16
 
 /* status codes */
@@ -377,6 +377,37 @@ typedef struct kge_conve {
 } kge_conve_t;
 int64_t kge_conve_trunk_workspace_bytes(const kge_conve_t* p, int64_t Q);
 int kge_conve_trunk_fwd(const kge_conve_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
+                        void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- HypER trunk, inference mode -----------------------------------------------------------
+ * HypER.forward up to the x.E^T product (pykg2vec/models/projection.py:581-606) with
+ * self.training == False: dropouts are identities and bn0 / bn1 / bn2 use their running statistics.
+ * Per query q (one relation-generated filter bank per query, a hypernetwork):
+ *   v = bn0(ent[e[q]])                                  [de]
+ *   w = fc1(rel[r[q]]) viewed [32][9]                   channel c uses w[9c .. 9c+8]
+ *   f[c][j] = bn1_c(sum_{t<9} w[c][t] * v[j+t])          j < de-8; no conv bias, no ReLU
+ *   x[q,:] = relu(bn2(fc(f flattened channel-major)))
+ * `direction` does not enter: the head direction passes (t, r) (no reciprocal relations).
+ * All pointers are device fp32 tensors with the reference's state_dict shapes:
+ *   ent [N,de], rel [num_rel,dr], bn0_* [1], fc1_weight [288,dr], fc1_bias [288], bn1_* [32],
+ *   fc_weight [de, F], fc_bias [de], bn2_* [de], F = 32 * (de - 8).
+ * The filters of all num_rel relations are computed on every call (one GEMM of num_rel x 288 x dr).
+ * x is [Q,de]; workspace >= kge_hyper_trunk_workspace_bytes() bytes (filter table, flattened
+ * feature maps and the Linear layer's slice partials).  Q = 0 is a no-op (e, r and x may then be NULL).
+ * KGE_ENOTSUP when de < 9 or the entity row does not fit the feature kernel's shared memory (de > 4096). */
+typedef struct kge_hyper {
+  int32_t ent_hidden_size, rel_hidden_size;
+  int64_t num_rel;
+  float bn0_eps, bn1_eps, bn2_eps;
+  const float* ent; const float* rel;
+  const float* bn0_weight; const float* bn0_bias; const float* bn0_mean; const float* bn0_var;
+  const float* fc1_weight; const float* fc1_bias;
+  const float* bn1_weight; const float* bn1_bias; const float* bn1_mean; const float* bn1_var;
+  const float* fc_weight; const float* fc_bias;
+  const float* bn2_weight; const float* bn2_bias; const float* bn2_mean; const float* bn2_var;
+} kge_hyper_t;
+int64_t kge_hyper_trunk_workspace_bytes(const kge_hyper_t* p, int64_t Q);
+int kge_hyper_trunk_fwd(const kge_hyper_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
                         void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- negative sampling on the device: replaces the CPU sampler processes ----

@@ -38,6 +38,7 @@ MODEL_MAP = {
     "convkb": ("pykg2vec_b200.pointwise", "ConvKB"),
     "conve": ("pykg2vec_b200.projection", "ConvE"),
     "tucker": ("pykg2vec_b200.projection", "TuckER"),
+    "hyper": ("pykg2vec_b200.projection", "HypER"),
 }
 
 

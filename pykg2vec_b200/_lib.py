@@ -11,7 +11,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_build", "libkge_b200.so")
 MAX_TABLES = 16
-ABI_VERSION = 5
+ABI_VERSION = 6
 ENOTSUP = -2   # include/kge_b200.h KGE_ENOTSUP
 
 MODEL_IDS = {
@@ -32,7 +32,8 @@ EXPORTS = [
     "kge_rank_workspace_bytes", "kge_rank_1vsall", "kge_rank_tc_probe", "kge_rank_last_sweep_ms", "kge_rank_last_sweep_directions", "kge_debug_set_tc_trace",
     "kge_tripleset_capacity", "kge_tripleset_build", "kge_sample_negatives",
     "kge_proj_tail_fwd", "kge_proj_tail_bwd", "kge_proj_bce", "kge_proj_rank_workspace_bytes", "kge_proj_rank", "kge_proj_labels",
-    "kge_conve_trunk_workspace_bytes", "kge_conve_trunk_fwd", "kge_project_entities", "kge_normalize_rows_to",
+    "kge_conve_trunk_workspace_bytes", "kge_conve_trunk_fwd", "kge_hyper_trunk_workspace_bytes", "kge_hyper_trunk_fwd",
+    "kge_project_entities", "kge_normalize_rows_to",
 ]
 
 
@@ -74,6 +75,7 @@ def lib():
     L.kge_tripleset_capacity.restype = ctypes.c_int64
     L.kge_proj_rank_workspace_bytes.restype = ctypes.c_int64
     L.kge_conve_trunk_workspace_bytes.restype = ctypes.c_int64
+    L.kge_hyper_trunk_workspace_bytes.restype = ctypes.c_int64
     if L.kge_abi_version() != ABI_VERSION:
         raise KgeError("libkge_b200.so ABI %d != binding ABI %d" % (L.kge_abi_version(), ABI_VERSION))
     _lib = L
@@ -528,6 +530,56 @@ def conve_trunk_fwd(model, e, r, out=None):
         out = torch.empty((Q, p.hidden_size), dtype=torch.float32, device=e.device)
     check(lib().kge_conve_trunk_fwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), _ptr(out), _ptr(ws),
                                     ctypes.c_int64(ws.numel()), _stream()), "kge_conve_trunk_fwd")
+    return out
+
+
+HYPER_FIELDS = ("ent", "rel", "bn0_weight", "bn0_bias", "bn0_mean", "bn0_var", "fc1_weight", "fc1_bias",
+                "bn1_weight", "bn1_bias", "bn1_mean", "bn1_var", "fc_weight", "fc_bias",
+                "bn2_weight", "bn2_bias", "bn2_mean", "bn2_var")
+
+
+class KgeHyper(ctypes.Structure):
+    """kge_hyper_t of include/kge_b200.h."""
+    _fields_ = [("ent_hidden_size", ctypes.c_int32), ("rel_hidden_size", ctypes.c_int32), ("num_rel", ctypes.c_int64),
+                ("bn0_eps", ctypes.c_float), ("bn1_eps", ctypes.c_float), ("bn2_eps", ctypes.c_float)] + \
+               [(n, ctypes.c_void_p) for n in HYPER_FIELDS]
+
+
+def hyper_trunk_workspace_bytes(ent_hidden_size, rel_hidden_size, num_rel, Q):
+    """bytes of device workspace kge_hyper_trunk_fwd needs for Q queries (0 for an unsupported shape)"""
+    p = KgeHyper()
+    p.ent_hidden_size, p.rel_hidden_size, p.num_rel = int(ent_hidden_size), int(rel_hidden_size), int(num_rel)
+    return int(lib().kge_hyper_trunk_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q)))
+
+
+def hyper_trunk_fwd(model, e, r, out=None, workspace=None):
+    """HypER inference trunk (projection.py:581-606, eval mode): x [Q,de] for entity ids e and relation ids r
+    (both directions pass their own (entity, relation) pair: HypER has no reciprocal relations).  `model` is a
+    HypER with the reference's sub-module names.  `workspace`: optional uint8 device buffer, grown if too small."""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    if r.numel() != Q:
+        raise KgeError("e and r must have equal length")
+    mods = {"bn0": model.bn0, "bn1": model.bn1, "bn2": model.bn2}
+    tensors = {"ent": model.ent_embeddings.weight, "rel": model.rel_embeddings.weight,
+               "fc1_weight": model.fc1.weight, "fc1_bias": model.fc1.bias,
+               "fc_weight": model.fc.weight, "fc_bias": model.fc.bias}
+    for name, bn in mods.items():
+        tensors.update({name + "_weight": bn.weight, name + "_bias": bn.bias,
+                        name + "_mean": bn.running_mean, name + "_var": bn.running_var})
+    p = KgeHyper()
+    p.ent_hidden_size, p.rel_hidden_size = int(model.ent_hidden_size), int(model.rel_hidden_size)
+    p.num_rel = int(model.rel_embeddings.weight.shape[0])
+    p.bn0_eps, p.bn1_eps, p.bn2_eps = float(model.bn0.eps), float(model.bn1.eps), float(model.bn2.eps)
+    for name in HYPER_FIELDS:
+        setattr(p, name, _dev_f32(tensors[name].detach(), name).data_ptr())
+    nbytes = int(lib().kge_hyper_trunk_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q)))
+    if workspace is None or workspace.numel() < nbytes:
+        workspace = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=e.device)
+    if out is None:
+        out = torch.empty((Q, p.ent_hidden_size), dtype=torch.float32, device=e.device)
+    check(lib().kge_hyper_trunk_fwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), _ptr(out), _ptr(workspace),
+                                    ctypes.c_int64(workspace.numel()), _stream()), "kge_hyper_trunk_fwd")
     return out
 
 

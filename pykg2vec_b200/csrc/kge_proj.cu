@@ -1,10 +1,10 @@
 // kge_proj.cu — C-ABI launchers of the projection-model tail (kernels and launch plans:
-// kge_proj.cuh) and of ConvE's inference trunk (kge_conve.cuh, which reuses the same tiled GEMM —
-// one translation unit so the kernel template is instantiated once).  Declarations and reference
-// citations: include/kge_b200.h.
+// kge_proj.cuh) and of the ConvE and HypER inference trunks (kge_conve.cuh, kge_hyper.cuh, which
+// reuse the same tiled GEMM — one translation unit so the kernel template is instantiated once).
+// Declarations and reference citations: include/kge_b200.h.
 #include <cstdlib>
 
-#include "kge_conve.cuh"
+#include "kge_hyper.cuh"
 
 using namespace kge;
 
@@ -177,6 +177,72 @@ int kge_conve_trunk_fwd(const kge_conve_t* p, const int64_t* e, const int64_t* r
   conve_fc_combine_kernel<<<proj_tiles(Q * k, 256), 256, 0, st>>>(partial, conve_fc_slices(F), Q * k, k,
                                                                  p->fc_bias, x);
   KGE_CHECK_LAUNCH("conve_fc_combine_kernel");
+  return KGE_OK;
+}
+
+
+// ---- HypER inference trunk ----------------------------------------------------------------
+
+static bool hyper_shape_ok(const kge_hyper_t* p) {
+  return p && p->ent_hidden_size >= HYPER_FW && p->ent_hidden_size <= HYPER_MAX_DE && p->rel_hidden_size > 0 &&
+         p->num_rel > 0;
+}
+
+int64_t kge_hyper_trunk_workspace_bytes(const kge_hyper_t* p, int64_t Q) {
+  if (!hyper_shape_ok(p)) return 0;
+  return hyper_layout(p->num_rel, Q > 0 ? Q : 1, p->ent_hidden_size).total * (int64_t)sizeof(float);
+}
+
+int kge_hyper_trunk_fwd(const kge_hyper_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
+                        void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!p || !workspace || (Q > 0 && (!e || !r || !x))) {   // an empty batch may pass null id / output pointers
+    set_error("kge_hyper_trunk_fwd: null pointer");
+    return KGE_EINVAL;
+  }
+  const int de = p->ent_hidden_size, dr = p->rel_hidden_size;
+  if (de < HYPER_FW || de > HYPER_MAX_DE) {
+    set_error("kge_hyper_trunk_fwd: unsupported ent_hidden_size %d (needs %d <= de <= %d)", de, HYPER_FW,
+              HYPER_MAX_DE);
+    return KGE_ENOTSUP;
+  }
+  if (dr <= 0 || p->num_rel <= 0 || (p->num_rel + PBM - 1) / PBM > 65535) {
+    set_error("kge_hyper_trunk_fwd: bad rel_hidden_size %d / num_rel %lld", dr, (long long)p->num_rel);
+    return KGE_EINVAL;
+  }
+  const float* ptrs[] = {p->ent, p->rel, p->bn0_weight, p->bn0_bias, p->bn0_mean, p->bn0_var, p->fc1_weight,
+                         p->fc1_bias, p->bn1_weight, p->bn1_bias, p->bn1_mean, p->bn1_var, p->fc_weight, p->fc_bias,
+                         p->bn2_weight, p->bn2_bias, p->bn2_mean, p->bn2_var};
+  for (const float* t : ptrs)
+    if (!t) { set_error("kge_hyper_trunk_fwd: null parameter tensor"); return KGE_EINVAL; }
+  if (Q < 0 || (Q + PBM - 1) / PBM > 65535) { set_error("kge_hyper_trunk_fwd: bad Q"); return KGE_EINVAL; }
+  if (workspace_bytes < kge_hyper_trunk_workspace_bytes(p, Q)) {
+    set_error("kge_hyper_trunk_fwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  if (Q == 0) return KGE_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const HyperLayout lay = hyper_layout(p->num_rel, Q, de);
+  float* ws = (float*)workspace;
+  if (int rc = launch_gemm<EPI_STORE>(hyper_plan_filters(p->rel, p->fc1_weight, p->fc1_bias, p->num_rel, dr,
+                                                         ws + lay.filt), st, "proj_gemm_kernel<hyper filters>"))
+    return rc;
+  HyperFeat f{};
+  f.ent = p->ent; f.filt = ws + lay.filt; f.e = e; f.r = r; f.de = de;
+  f.bn0_w = p->bn0_weight; f.bn0_b = p->bn0_bias; f.bn0_mean = p->bn0_mean; f.bn0_var = p->bn0_var;
+  f.bn0_eps = p->bn0_eps;
+  f.bn1_w = p->bn1_weight; f.bn1_b = p->bn1_bias; f.bn1_mean = p->bn1_mean; f.bn1_var = p->bn1_var;
+  f.bn1_eps = p->bn1_eps;
+  f.feat = ws + lay.feat;
+  hyper_feature_kernel<<<(unsigned)Q, HYPER_THREADS, 0, st>>>(f);
+  KGE_CHECK_LAUNCH("hyper_feature_kernel");
+  const long long F = hyper_feat_width(de);
+  float* partial = ws + lay.partial;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_fc(f.feat, p->fc_weight, Q, F, de, partial), st,
+                                      "proj_gemm_kernel<hyper fc>")) return rc;
+  hyper_fc_combine_kernel<<<proj_tiles(Q * de, 256), 256, 0, st>>>(partial, conve_fc_slices(F), Q * de, de, p->fc_bias,
+                                                                   p->bn2_weight, p->bn2_bias, p->bn2_mean,
+                                                                   p->bn2_var, p->bn2_eps, x);
+  KGE_CHECK_LAUNCH("hyper_fc_combine_kernel");
   return KGE_OK;
 }
 

@@ -15,6 +15,12 @@ ReLU on a [b, 1, 2*h2, h1] image) runs in two ways:
   * evaluation (`proj_query`, used by the batched Evaluator): kge_conve_trunk_fwd — gather +
     BN0 + conv + BN1 + ReLU in one kernel and the Linear layer through the same tiled GEMM as the
     tail.
+
+HypER (projection.py:508-618) has the same tail and loss; its trunk convolves the BatchNormed entity
+row with 32 filters of width 9 that a Linear layer (fc1) generates from the query's relation.  Training
+runs the reference's layers (the per-query filters as one grouped convolution, TF32 off); evaluation
+without autograd runs kge_hyper_trunk_fwd — one GEMM for every relation's filters, one kernel for
+gather + bn0 + conv + bn1, the Linear layer on the tail's tiled GEMM, then bn2 + ReLU.
 """
 import torch
 import torch.nn as nn
@@ -181,6 +187,92 @@ class TuckER(ProjectionModel):
 
     def forward(self, e1, r, direction="head"):
         return ProjTailFunction.apply(self.proj_query(e1, r, direction), self.ent_embeddings.weight, None)
+
+    def predict_tail_rank(self, e, r, topk=-1):
+        _, rank = torch.topk(-self.forward(e, r, direction="tail"), k=topk)
+        return rank
+
+    def predict_head_rank(self, e, r, topk=-1):
+        _, rank = torch.topk(-self.forward(e, r, direction="head"), k=topk)
+        return rank
+
+
+class HypER(ProjectionModel):
+    """pykg2vec/models/projection.py:508-618 — same kwargs (including the required `device`), sub-module
+    names (state_dict keys b / ent_embeddings / rel_embeddings / bn0 / bn1 / bn2 / fc / fc1, padding_idx=0 on
+    both embeddings), parameter_list and loss binding.  As in the reference `direction` is validated and
+    otherwise ignored: the head direction runs the same function on (t, r)."""
+
+    def __init__(self, **kwargs):
+        super(HypER, self).__init__(self.__class__.__name__.lower())
+        param_list = ["tot_entity", "tot_relation", "ent_hidden_size", "rel_hidden_size", "input_dropout",
+                      "hidden_dropout", "feature_map_dropout"]
+        param_dict = self.load_params(param_list, kwargs)
+        self.__dict__.update(param_dict)
+        self.device = kwargs["device"]
+        self.filt_h, self.filt_w = 1, 9
+        self.in_channels, self.out_channels = 1, 32
+        de, dr = self.ent_hidden_size, self.rel_hidden_size
+        self.ent_embeddings = NamedEmbedding("ent_embeddings", self.tot_entity, de, padding_idx=0)
+        self.rel_embeddings = NamedEmbedding("rel_embeddings", self.tot_relation, dr, padding_idx=0)
+        self.inp_drop = nn.Dropout(self.input_dropout)
+        self.hidden_drop = nn.Dropout(self.hidden_dropout)
+        self.feature_map_drop = nn.Dropout2d(self.feature_map_dropout)
+        self.bn0 = nn.BatchNorm2d(self.in_channels)
+        self.bn1 = nn.BatchNorm2d(self.out_channels)
+        self.bn2 = nn.BatchNorm1d(de)
+        self.register_parameter("b", nn.Parameter(torch.zeros(self.tot_entity)))
+        self.fc = nn.Linear((1 - self.filt_h + 1) * (de - self.filt_w + 1) * self.out_channels, de)
+        self.fc1 = nn.Linear(dr, self.in_channels * self.out_channels * self.filt_h * self.filt_w)
+        nn.init.xavier_uniform_(self.ent_embeddings.weight.data)
+        nn.init.xavier_uniform_(self.rel_embeddings.weight.data)
+        self.parameter_list = [self.ent_embeddings, self.rel_embeddings]
+        self.loss = Criterion.multi_class_bce
+
+    def embed(self, h, r, t):
+        return self.ent_embeddings(h), self.rel_embeddings(r), self.ent_embeddings(t)
+
+    def embed2(self, e, r):
+        return self.ent_embeddings(e), self.rel_embeddings(r)
+
+    # ---- trunk: HypER.forward before the x . E^T product (projection.py:583-606) ----
+    def _trunk_layers(self, e, r):
+        e_emb, r_emb = self.embed2(e, r)
+        B, de = e_emb.size(0), self.ent_embeddings.weight.size(1)
+        x = self.bn0(e_emb.view(-1, 1, 1, de))
+        x = self.inp_drop(x)
+        k = self.fc1(r_emb)
+        k = k.view(-1, self.in_channels, self.out_channels, self.filt_h, self.filt_w)
+        k = k.view(B * self.in_channels * self.out_channels, 1, self.filt_h, self.filt_w)
+        x = x.permute(1, 0, 2, 3)
+        # one group per query: query i's 32 filters see only its own row (TF32 off, see _Fp32Conv2d)
+        x = _Fp32Conv2d.apply(x, k, None, (1, 1), (0, 0), (1, 1), B)
+        x = x.view(B, 1, self.out_channels, 1 - self.filt_h + 1, de - self.filt_w + 1)
+        x = x.permute(0, 3, 4, 1, 2)
+        x = torch.sum(x, dim=3)
+        x = x.permute(0, 3, 1, 2).contiguous()
+        x = self.bn1(x)
+        x = self.feature_map_drop(x)
+        x = x.view(B, -1)
+        x = self.fc(x)
+        x = self.hidden_drop(x)
+        x = self.bn2(x)   # applied in both modes (unlike ConvE)
+        return torch.relu(x)
+
+    def proj_query(self, e, r, direction="tail"):
+        """x [b, de]: the operand of the tail product, for the batched Evaluator (eval mode)."""
+        assert direction in ("head", "tail"), "Unknown forward direction"
+        _require_cuda(e, r, self.ent_embeddings.weight)
+        if not self.training and not torch.is_grad_enabled():
+            return _lib.hyper_trunk_fwd(self, e.contiguous(), r.contiguous())
+        return self._trunk_layers(e, r)
+
+    def proj_tail_tables(self):
+        """(entity table [N,de], bias row [N]) of the tail product."""
+        return self.ent_embeddings.weight, self.b
+
+    def forward(self, e, r, direction="tail"):
+        return ProjTailFunction.apply(self.proj_query(e, r, direction), self.ent_embeddings.weight, self.b)
 
     def predict_tail_rank(self, e, r, topk=-1):
         _, rank = torch.topk(-self.forward(e, r, direction="tail"), k=topk)
