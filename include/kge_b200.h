@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KGE_ABI_VERSION 6
+#define KGE_ABI_VERSION 7
 #define KGE_MAX_TABLES 16
 
 /* status codes */
@@ -409,6 +409,42 @@ typedef struct kge_hyper {
 int64_t kge_hyper_trunk_workspace_bytes(const kge_hyper_t* p, int64_t Q);
 int kge_hyper_trunk_fwd(const kge_hyper_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
                         void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- InteractE trunk, inference mode -------------------------------------------------------
+ * InteractE.forward up to the x.E^T product (pykg2vec/models/projection.py:425-442) with
+ * self.training == False: dropouts are identities and bn0 / bn1 / bn2 use their running statistics.
+ * P = feature_permutation, F = num_filters, ks = kernel_size, H = 2*reshape_width image rows,
+ * W = reshape_height image columns, k = reshape_width*reshape_height, pad = ks/2.  Per query q:
+ *   comb = [ent[e[q]] ; rel[r[q]]]                                  [2k]
+ *   img[p][i][j] = bn0_p(comb[perm[p][i*W + j]])                    P chequer-permuted images [H][W]
+ *   f[p*F+f][i][j] = relu(bn1_{p*F+f}(sum_{u,v<ks} conv_filt[f][u][v] * img[p][(i+u-pad) mod H][(j+v-pad) mod W]))
+ *   x[q,:] = relu(bn2(fc(f flattened channel-major)))
+ * (circular padding, filter f on every image, no conv bias).  `direction` does not enter: the head direction
+ * passes (t, r) (no reciprocal relations).  perm is the model's chequer permutation, int64 [P, 2k] on the device.
+ * The other pointers are device fp32 tensors with the reference's state_dict shapes:
+ *   ent [N,k], rel [num_rel,k], bn0_* [P], conv_filt [F,1,ks,ks], bn1_* [P*F], fc_weight [k, P*F*H*W],
+ *   fc_bias [k], bn2_* [k].
+ * x is [Q,k]; workspace >= kge_interacte_trunk_workspace_bytes() bytes (the flattened feature maps and the
+ * Linear layer's slice partials, ~(P*F*H*W + ceil(P*F*H*W / 512) * k) floats per query, 214 KB at the default
+ * (1, 96, 9, 20x10) shape: callers bound it by splitting Q).  Q = 0 is a no-op (e, r and x may then be NULL).
+ * KGE_ENOTSUP for an even ks or ks < 3 (the reference's forward fails there), pad > min(H, W), or when the
+ * filter bank (ks*ks*ceil8(F) floats), the bn1 folds (2*P*ceil8(F)) and the P padded images
+ * ((H+2pad)*(W+2pad) each) exceed 227 KB, the per-block shared memory of sm_90. */
+typedef struct kge_interacte {
+  int32_t feature_permutation, num_filters, kernel_size, reshape_height, reshape_width;
+  int64_t num_rel;
+  float bn0_eps, bn1_eps, bn2_eps;
+  const int64_t* perm;
+  const float* ent; const float* rel;
+  const float* bn0_weight; const float* bn0_bias; const float* bn0_mean; const float* bn0_var;
+  const float* conv_filt;
+  const float* bn1_weight; const float* bn1_bias; const float* bn1_mean; const float* bn1_var;
+  const float* fc_weight; const float* fc_bias;
+  const float* bn2_weight; const float* bn2_bias; const float* bn2_mean; const float* bn2_var;
+} kge_interacte_t;
+int64_t kge_interacte_trunk_workspace_bytes(const kge_interacte_t* p, int64_t Q);
+int kge_interacte_trunk_fwd(const kge_interacte_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
+                            void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- negative sampling on the device: replaces the CPU sampler processes ----
  * process_function_pairwise / process_function_pointwise (pykg2vec/data/generator.py:42-158).

@@ -39,6 +39,7 @@ MODEL_MAP = {
     "conve": ("pykg2vec_b200.projection", "ConvE"),
     "tucker": ("pykg2vec_b200.projection", "TuckER"),
     "hyper": ("pykg2vec_b200.projection", "HypER"),
+    "interacte": ("pykg2vec_b200.projection", "InteractE"),
 }
 
 

@@ -11,7 +11,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_build", "libkge_b200.so")
 MAX_TABLES = 16
-ABI_VERSION = 6
+ABI_VERSION = 7
 ENOTSUP = -2   # include/kge_b200.h KGE_ENOTSUP
 
 MODEL_IDS = {
@@ -33,6 +33,7 @@ EXPORTS = [
     "kge_tripleset_capacity", "kge_tripleset_build", "kge_sample_negatives",
     "kge_proj_tail_fwd", "kge_proj_tail_bwd", "kge_proj_bce", "kge_proj_rank_workspace_bytes", "kge_proj_rank", "kge_proj_labels",
     "kge_conve_trunk_workspace_bytes", "kge_conve_trunk_fwd", "kge_hyper_trunk_workspace_bytes", "kge_hyper_trunk_fwd",
+    "kge_interacte_trunk_workspace_bytes", "kge_interacte_trunk_fwd",
     "kge_project_entities", "kge_normalize_rows_to",
 ]
 
@@ -76,6 +77,7 @@ def lib():
     L.kge_proj_rank_workspace_bytes.restype = ctypes.c_int64
     L.kge_conve_trunk_workspace_bytes.restype = ctypes.c_int64
     L.kge_hyper_trunk_workspace_bytes.restype = ctypes.c_int64
+    L.kge_interacte_trunk_workspace_bytes.restype = ctypes.c_int64
     if L.kge_abi_version() != ABI_VERSION:
         raise KgeError("libkge_b200.so ABI %d != binding ABI %d" % (L.kge_abi_version(), ABI_VERSION))
     _lib = L
@@ -580,6 +582,84 @@ def hyper_trunk_fwd(model, e, r, out=None, workspace=None):
         out = torch.empty((Q, p.ent_hidden_size), dtype=torch.float32, device=e.device)
     check(lib().kge_hyper_trunk_fwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), _ptr(out), _ptr(workspace),
                                     ctypes.c_int64(workspace.numel()), _stream()), "kge_hyper_trunk_fwd")
+    return out
+
+
+INTERACTE_FIELDS = ("ent", "rel", "bn0_weight", "bn0_bias", "bn0_mean", "bn0_var", "conv_filt",
+                    "bn1_weight", "bn1_bias", "bn1_mean", "bn1_var", "fc_weight", "fc_bias",
+                    "bn2_weight", "bn2_bias", "bn2_mean", "bn2_var")
+# upper bound of the workspace one kge_interacte_trunk_fwd call may use: the features alone take 150 KB per
+# query at the default shape (1, 96, 9, 20x10), 400 KB at (4, 64, 7, 20x10), so a large batch is split into
+# chunks of queries (independent of each other: the result is the same bits as one call)
+INTERACTE_WORKSPACE_CAP = 256 << 20
+
+
+class KgeInteracte(ctypes.Structure):
+    """kge_interacte_t of include/kge_b200.h."""
+    _fields_ = [("feature_permutation", ctypes.c_int32), ("num_filters", ctypes.c_int32),
+                ("kernel_size", ctypes.c_int32), ("reshape_height", ctypes.c_int32),
+                ("reshape_width", ctypes.c_int32), ("num_rel", ctypes.c_int64),
+                ("bn0_eps", ctypes.c_float), ("bn1_eps", ctypes.c_float), ("bn2_eps", ctypes.c_float),
+                ("perm", ctypes.c_void_p)] + [(n, ctypes.c_void_p) for n in INTERACTE_FIELDS]
+
+
+def interacte_struct(P, F, ks, reshape_height, reshape_width, num_rel):
+    """a KgeInteracte holding the geometry only (pointers NULL)"""
+    p = KgeInteracte()
+    p.feature_permutation, p.num_filters, p.kernel_size = int(P), int(F), int(ks)
+    p.reshape_height, p.reshape_width, p.num_rel = int(reshape_height), int(reshape_width), int(num_rel)
+    return p
+
+
+def interacte_trunk_workspace_bytes(P, F, ks, reshape_height, reshape_width, num_rel, Q):
+    """bytes of device workspace ONE kge_interacte_trunk_fwd call needs for Q queries (0 for an unsupported
+    shape)"""
+    p = interacte_struct(P, F, ks, reshape_height, reshape_width, num_rel)
+    return int(lib().kge_interacte_trunk_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q)))
+
+
+def interacte_trunk_fwd(model, e, r, out=None, workspace=None, cap=None, perm=None):
+    """InteractE inference trunk (projection.py:425-442, eval mode): x [Q,k] for entity ids e and relation ids r
+    (both directions pass their own (entity, relation) pair: InteractE has no reciprocal relations).  `model` is
+    an InteractE with the reference's sub-module names; its chequer permutation is model.chequer_perm.  The
+    queries run in chunks whose workspace stays under `cap` bytes (default INTERACTE_WORKSPACE_CAP; a single
+    query always runs).  `workspace`: optional uint8 device buffer, grown if too small.  `perm`: the chequer
+    permutation already on e's device (default: model.chequer_perm, copied there if needed)."""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    if r.numel() != Q:
+        raise KgeError("e and r must have equal length")
+    mods = {"bn0": model.bn0, "bn1": model.bn1, "bn2": model.bn2}
+    tensors = {"ent": model.ent_embeddings.weight, "rel": model.rel_embeddings.weight, "conv_filt": model.conv_filt,
+               "fc_weight": model.fc.weight, "fc_bias": model.fc.bias}
+    for name, bn in mods.items():
+        tensors.update({name + "_weight": bn.weight, name + "_bias": bn.bias,
+                        name + "_mean": bn.running_mean, name + "_var": bn.running_var})
+    p = interacte_struct(model.feature_permutation, model.num_filters, model.kernel_size, model.reshape_height,
+                         model.reshape_width, model.rel_embeddings.weight.shape[0])
+    p.bn0_eps, p.bn1_eps, p.bn2_eps = float(model.bn0.eps), float(model.bn1.eps), float(model.bn2.eps)
+    for name in INTERACTE_FIELDS:
+        setattr(p, name, _dev_f32(tensors[name].detach(), name).data_ptr())
+    perm = model.chequer_perm if perm is None else perm
+    if perm.device != e.device or perm.dtype != torch.int64:
+        perm = perm.to(device=e.device, dtype=torch.int64)
+    p.perm = _dev_i64(perm.contiguous(), "chequer_perm").data_ptr()
+    k = int(model.reshape_width) * int(model.reshape_height)
+    if out is None:
+        out = torch.empty((Q, k), dtype=torch.float32, device=e.device)
+    per_query = int(lib().kge_interacte_trunk_workspace_bytes(ctypes.byref(p), ctypes.c_int64(1)))
+    if per_query == 0:    # unsupported shape: the call below reports why
+        chunk = max(Q, 1)
+    else:
+        chunk = max(1, min(max(Q, 1), int(INTERACTE_WORKSPACE_CAP if cap is None else cap) // per_query))
+    nbytes = int(lib().kge_interacte_trunk_workspace_bytes(ctypes.byref(p), ctypes.c_int64(chunk)))
+    if workspace is None or workspace.numel() < nbytes:
+        workspace = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=e.device)
+    for q0 in range(0, max(Q, 1), chunk):
+        n = min(chunk, Q - q0)
+        check(lib().kge_interacte_trunk_fwd(ctypes.byref(p), _ptr(e[q0:q0 + n]), _ptr(r[q0:q0 + n]),
+                                            ctypes.c_int64(n), _ptr(out[q0:q0 + n]), _ptr(workspace),
+                                            ctypes.c_int64(workspace.numel()), _stream()), "kge_interacte_trunk_fwd")
     return out
 
 

@@ -1,10 +1,10 @@
 // kge_proj.cu — C-ABI launchers of the projection-model tail (kernels and launch plans:
-// kge_proj.cuh) and of the ConvE and HypER inference trunks (kge_conve.cuh, kge_hyper.cuh, which
-// reuse the same tiled GEMM — one translation unit so the kernel template is instantiated once).
-// Declarations and reference citations: include/kge_b200.h.
+// kge_proj.cuh) and of the ConvE, HypER and InteractE inference trunks (kge_conve.cuh, kge_hyper.cuh,
+// kge_interacte.cuh, which reuse the same tiled GEMM — one translation unit so the kernel template is
+// instantiated once).  Declarations and reference citations: include/kge_b200.h.
 #include <cstdlib>
 
-#include "kge_hyper.cuh"
+#include "kge_interacte.cuh"
 
 using namespace kge;
 
@@ -242,6 +242,94 @@ int kge_hyper_trunk_fwd(const kge_hyper_t* p, const int64_t* e, const int64_t* r
   hyper_fc_combine_kernel<<<proj_tiles(Q * de, 256), 256, 0, st>>>(partial, conve_fc_slices(F), Q * de, de, p->fc_bias,
                                                                    p->bn2_weight, p->bn2_bias, p->bn2_mean,
                                                                    p->bn2_var, p->bn2_eps, x);
+  KGE_CHECK_LAUNCH("hyper_fc_combine_kernel");
+  return KGE_OK;
+}
+
+
+// ---- InteractE inference trunk ------------------------------------------------------------
+
+// KGE_OK, or the error code of an unsupported / malformed geometry (message set for `fn`)
+static int interacte_shape(const kge_interacte_t* p, const char* fn) {
+  const int P = p->feature_permutation, F = p->num_filters, ks = p->kernel_size;
+  const int H = 2 * p->reshape_width, W = p->reshape_height;
+  if (P <= 0 || F <= 0 || ks <= 0 || p->reshape_width <= 0 || W <= 0 || p->num_rel <= 0 ||
+      (long long)H * W > (1 << 20)) {
+    set_error("%s: bad geometry P=%d F=%d ks=%d reshape %dx%d num_rel %lld", fn, P, F, ks, p->reshape_height,
+              p->reshape_width, (long long)p->num_rel);
+    return KGE_EINVAL;
+  }
+  if (ks < 3 || ks % 2 == 0 || ks / 2 > (H < W ? H : W)) {
+    set_error("%s: unsupported kernel_size %d on a %dx%d image (needs an odd ks >= 3, ks/2 <= %d)", fn, ks, H, W,
+              H < W ? H : W);
+    return KGE_ENOTSUP;
+  }
+  const long long smem = interacte_smem(P, F, ks, H, W).total * (long long)sizeof(float);
+  if (smem > INTERACTE_SMEM_MAX) {
+    set_error("%s: filter bank + %d padded images need %lld bytes of shared memory (max %d)", fn, P, smem,
+              INTERACTE_SMEM_MAX);
+    return KGE_ENOTSUP;
+  }
+  const long long Fw = interacte_feat_width(P, F, H, W);
+  if (Fw > (1ll << 30) || conve_fc_slices(Fw) > 65535) {
+    set_error("%s: %lld features per query exceed the Linear layer's GEMM", fn, Fw);
+    return KGE_ENOTSUP;
+  }
+  return KGE_OK;
+}
+
+int64_t kge_interacte_trunk_workspace_bytes(const kge_interacte_t* p, int64_t Q) {
+  if (!p || interacte_shape(p, "kge_interacte_trunk_workspace_bytes")) return 0;
+  return interacte_layout(Q > 0 ? Q : 1, p->feature_permutation, p->num_filters, 2 * p->reshape_width,
+                          p->reshape_height).total * (int64_t)sizeof(float);
+}
+
+int kge_interacte_trunk_fwd(const kge_interacte_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
+                            void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!p || !workspace || (Q > 0 && (!e || !r || !x))) {   // an empty batch may pass null id / output pointers
+    set_error("kge_interacte_trunk_fwd: null pointer");
+    return KGE_EINVAL;
+  }
+  if (int rc = interacte_shape(p, "kge_interacte_trunk_fwd")) return rc;
+  const float* ptrs[] = {p->ent, p->rel, p->bn0_weight, p->bn0_bias, p->bn0_mean, p->bn0_var, p->conv_filt,
+                         p->bn1_weight, p->bn1_bias, p->bn1_mean, p->bn1_var, p->fc_weight, p->fc_bias,
+                         p->bn2_weight, p->bn2_bias, p->bn2_mean, p->bn2_var};
+  for (const float* t : ptrs)
+    if (!t) { set_error("kge_interacte_trunk_fwd: null parameter tensor"); return KGE_EINVAL; }
+  if (!p->perm) { set_error("kge_interacte_trunk_fwd: null perm"); return KGE_EINVAL; }
+  if (Q < 0 || (Q + PBM - 1) / PBM > 65535) { set_error("kge_interacte_trunk_fwd: bad Q"); return KGE_EINVAL; }
+  if (workspace_bytes < kge_interacte_trunk_workspace_bytes(p, Q)) {
+    set_error("kge_interacte_trunk_fwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  if (Q == 0) return KGE_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int P = p->feature_permutation, F = p->num_filters, ks = p->kernel_size;
+  const int H = 2 * p->reshape_width, W = p->reshape_height, k = p->reshape_width * p->reshape_height;
+  const InteracteLayout lay = interacte_layout(Q, P, F, H, W);
+  float* ws = (float*)workspace;
+  InteracteFeat f{};
+  f.ent = p->ent; f.rel = p->rel; f.perm = p->perm; f.e = e; f.r = r;
+  f.P = P; f.F = F; f.ks = ks; f.H = H; f.W = W;
+  f.bn0_w = p->bn0_weight; f.bn0_b = p->bn0_bias; f.bn0_mean = p->bn0_mean; f.bn0_var = p->bn0_var;
+  f.bn0_eps = p->bn0_eps;
+  f.conv_filt = p->conv_filt;
+  f.bn1_w = p->bn1_weight; f.bn1_b = p->bn1_bias; f.bn1_mean = p->bn1_mean; f.bn1_var = p->bn1_var;
+  f.bn1_eps = p->bn1_eps;
+  f.feat = ws + lay.feat;
+  const size_t smem = (size_t)interacte_smem(P, F, ks, H, W).total * sizeof(float);
+  if (smem > 48 * 1024)
+    KGE_CUDA_OK(cudaFuncSetAttribute(interacte_feature_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                     (int)smem));
+  interacte_feature_kernel<<<(unsigned)Q, INTERACTE_THREADS, smem, st>>>(f);
+  KGE_CHECK_LAUNCH("interacte_feature_kernel");
+  const long long Fw = interacte_feat_width(P, F, H, W);
+  float* partial = ws + lay.partial;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_fc(f.feat, p->fc_weight, Q, Fw, k, partial), st,
+                                      "proj_gemm_kernel<interacte fc>")) return rc;
+  hyper_fc_combine_kernel<<<proj_tiles(Q * k, 256), 256, 0, st>>>(partial, conve_fc_slices(Fw), Q * k, k, p->fc_bias,
+                                                                  p->bn2_weight, p->bn2_bias, p->bn2_mean,
+                                                                  p->bn2_var, p->bn2_eps, x);
   KGE_CHECK_LAUNCH("hyper_fc_combine_kernel");
   return KGE_OK;
 }

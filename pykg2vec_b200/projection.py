@@ -21,7 +21,13 @@ row with 32 filters of width 9 that a Linear layer (fc1) generates from the quer
 runs the reference's layers (the per-query filters as one grouped convolution, TF32 off); evaluation
 without autograd runs kge_hyper_trunk_fwd — one GEMM for every relation's filters, one kernel for
 gather + bn0 + conv + bn1, the Linear layer on the tail's tiled GEMM, then bn2 + ReLU.
+
+InteractE (projection.py:347-505) has the same tail and loss; its trunk stacks P chequer-permuted images of the
+entity and relation features and convolves them circularly with one shared filter bank.  Training runs the
+reference's layers; evaluation without autograd runs kge_interacte_trunk_fwd — one kernel for gather +
+permutation + bn0 + circular conv + bn1 + ReLU, then HypER's Linear GEMM and bn2 + ReLU.
 """
+import numpy as np
 import torch
 import torch.nn as nn
 
@@ -187,6 +193,132 @@ class TuckER(ProjectionModel):
 
     def forward(self, e1, r, direction="head"):
         return ProjTailFunction.apply(self.proj_query(e1, r, direction), self.ent_embeddings.weight, None)
+
+    def predict_tail_rank(self, e, r, topk=-1):
+        _, rank = torch.topk(-self.forward(e, r, direction="tail"), k=topk)
+        return rank
+
+    def predict_head_rank(self, e, r, topk=-1):
+        _, rank = torch.topk(-self.forward(e, r, direction="head"), k=topk)
+        return rank
+
+
+def _chequer_perm(hidden_size, reshape_width, P):
+    """InteractE's chequer permutation [P, 2*hidden_size] (projection.py:468-505).  numpy draws, in this order,
+    P permutations of the entity features, then P of the relation features (np.random.permutation).  Image p
+    interleaves them pairwise, entity and relation (offset by hidden_size) features alternating; within every
+    run of reshape_width pairs the pair order is (entity, relation) when run index + p is even, else
+    (relation, entity)."""
+    ent = [np.random.permutation(hidden_size) for _ in range(P)]
+    rel = [np.random.permutation(hidden_size) for _ in range(P)]
+    run = np.arange(hidden_size) // reshape_width
+    rows = []
+    for p in range(P):
+        e, r = ent[p], rel[p] + hidden_size
+        ent_first = ((run + p) % 2 == 0)[:, None]
+        rows.append(np.where(ent_first, np.stack([e, r], 1), np.stack([r, e], 1)).reshape(-1))
+    return torch.from_numpy(np.stack(rows).astype(np.int64))
+
+
+class InteractE(ProjectionModel):
+    """pykg2vec/models/projection.py:347-505 — same kwargs (including the required `device`; hidden_size is read
+    and then replaced by reshape_width * reshape_height), sub-module names and state_dict keys (bias / conv_filt /
+    ent_embeddings / rel_embeddings / bn0 / bn1 / bn2 / fc), parameter_list and loss binding.  `chequer_perm`
+    (int64 [P, 2k]) is drawn from the global np.random at construction with the reference's calls and, as there,
+    is a plain attribute: not a parameter or buffer, so not in state_dict.  As in the reference `direction` is
+    validated and otherwise ignored: the head direction runs the same function on (t, r).
+
+    Training runs the reference's layers (the circular convolution through _Fp32Conv2d with TF32 off, so
+    conv_filt trains); evaluation without autograd runs kge_interacte_trunk_fwd — one kernel for gather +
+    permutation + bn0 + circular conv + bn1 + ReLU, the Linear layer on the tail's tiled GEMM, then bn2 + ReLU."""
+
+    def __init__(self, **kwargs):
+        super(InteractE, self).__init__(self.__class__.__name__.lower())
+        param_list = ["tot_entity", "tot_relation", "hidden_size", "input_dropout", "hidden_dropout",
+                      "feature_map_dropout", "feature_permutation", "num_filters", "kernel_size", "reshape_height",
+                      "reshape_width"]
+        param_dict = self.load_params(param_list, kwargs)
+        self.__dict__.update(param_dict)
+        self.hidden_size = self.reshape_width * self.reshape_height
+        self.device = kwargs["device"]
+        k, P = self.hidden_size, self.feature_permutation
+        # construction order = the reference's: it fixes the state_dict order and the torch / numpy draws
+        self.ent_embeddings = NamedEmbedding("ent_embeddings", self.tot_entity, k, padding_idx=None)
+        self.rel_embeddings = NamedEmbedding("rel_embeddings", self.tot_relation, k, padding_idx=None)
+        self.bceloss = nn.BCELoss()
+        self.inp_drop = nn.Dropout(self.input_dropout)
+        self.hidden_drop = nn.Dropout(self.hidden_dropout)
+        self.feature_map_drop = nn.Dropout2d(self.feature_map_dropout)
+        self.bn0 = nn.BatchNorm2d(P)
+        self.padding = 0
+        self.bn1 = nn.BatchNorm2d(self.num_filters * P)
+        self.flat_sz = self.reshape_height * 2 * self.reshape_width * self.num_filters * P
+        self.bn2 = nn.BatchNorm1d(k)
+        self.fc = nn.Linear(self.flat_sz, k)
+        self.chequer_perm = _chequer_perm(k, self.reshape_width, P).to(self.device)
+        self.register_parameter("bias", nn.Parameter(torch.zeros(self.tot_entity)))
+        self.register_parameter("conv_filt", nn.Parameter(torch.zeros(self.num_filters, 1, self.kernel_size,
+                                                                      self.kernel_size)))
+        nn.init.xavier_uniform_(self.ent_embeddings.weight)
+        nn.init.xavier_uniform_(self.rel_embeddings.weight)
+        nn.init.xavier_uniform_(self.conv_filt)
+        self.parameter_list = [self.ent_embeddings, self.rel_embeddings]
+        self.loss = Criterion.multi_class_bce
+        self._perm_dev = None
+
+    def embed(self, h, r, t):
+        return self.ent_embeddings(h), self.rel_embeddings(r), self.ent_embeddings(t)
+
+    def embed2(self, e, r):
+        return self.ent_embeddings(e), self.rel_embeddings(r)
+
+    def _perm_on(self, device):
+        """chequer_perm as int64 on `device`: copied once per (attribute value, device); the attribute itself stays
+        where construction (or the caller) put it"""
+        src = self.chequer_perm
+        if src.device == device and src.dtype == torch.int64:
+            return src
+        if self._perm_dev is None or self._perm_dev[0] is not src or self._perm_dev[1].device != device:
+            self._perm_dev = (src, src.to(device=device, dtype=torch.int64))
+        return self._perm_dev[1]
+
+    # ---- trunk: InteractE.forward before the x . E^T product (projection.py:427-442) ----
+    def _trunk_layers(self, e, r):
+        e_emb, r_emb = self.embed2(e, r)
+        comb = torch.cat([e_emb, r_emb], dim=-1)
+        H, W, P = 2 * self.reshape_width, self.reshape_height, self.feature_permutation
+        x = comb[:, self._perm_on(comb.device)].reshape(-1, P, H, W)
+        x = self.bn0(x)
+        x = self.inp_drop(x)
+        pad = self.kernel_size // 2
+        x = torch.cat([x[..., H - pad:, :], x, x[..., :pad, :]], dim=2)     # circular padding, rows then columns
+        x = torch.cat([x[..., W - pad:], x, x[..., :pad]], dim=3)
+        # filter f on every image: output channel p*F + f (TF32 off, see _Fp32Conv2d)
+        x = _Fp32Conv2d.apply(x, self.conv_filt.repeat(P, 1, 1, 1), None, (1, 1), (self.padding, self.padding),
+                              (1, 1), P)
+        x = self.bn1(x)
+        x = torch.relu(x)
+        x = self.feature_map_drop(x)
+        x = x.view(-1, self.flat_sz)
+        x = self.fc(x)
+        x = self.hidden_drop(x)
+        x = self.bn2(x)
+        return torch.relu(x)
+
+    def proj_query(self, e, r, direction="tail"):
+        """x [b, k]: the operand of the tail product, for the batched Evaluator (eval mode)."""
+        assert direction in ("head", "tail"), "Unknown forward direction"
+        _require_cuda(e, r, self.ent_embeddings.weight)
+        if not self.training and not torch.is_grad_enabled():
+            return _lib.interacte_trunk_fwd(self, e.contiguous(), r.contiguous(), perm=self._perm_on(e.device))
+        return self._trunk_layers(e, r)
+
+    def proj_tail_tables(self):
+        """(entity table [N,k], bias row [N]) of the tail product."""
+        return self.ent_embeddings.weight, self.bias
+
+    def forward(self, e, r, direction="tail"):
+        return ProjTailFunction.apply(self.proj_query(e, r, direction), self.ent_embeddings.weight, self.bias)
 
     def predict_tail_rank(self, e, r, topk=-1):
         _, rank = torch.topk(-self.forward(e, r, direction="tail"), k=topk)
