@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KGE_ABI_VERSION 7
+#define KGE_ABI_VERSION 8
 #define KGE_MAX_TABLES 16
 
 /* status codes */
@@ -445,6 +445,48 @@ typedef struct kge_interacte {
 int64_t kge_interacte_trunk_workspace_bytes(const kge_interacte_t* p, int64_t Q);
 int kge_interacte_trunk_fwd(const kge_interacte_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
                             void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- AcrE trunk, inference mode ------------------------------------------------------------
+ * AcrE.forward up to the x.E^T product (pykg2vec/models/projection.py:706-734) with self.training == False:
+ * dropouts are identities and bn0 / bn1 / bn2 use their running statistics.  C = in_channels, conv l is a
+ * 3x3 conv with stride 1 and padding = dilation = its atrous rate (zero padding: the maps stay 20 x 20).
+ * Per query q:
+ *   img[20][20] = bn0([ent[e[q]] ; rel[r[q]]])                      the two 200-wide rows, 10 x 20 each
+ *   serial (way 0):   y = conv3(conv2(conv1(img))) + img            1 -> C -> C -> C, img on every channel
+ *   parallel (way 1): y[c] = W_gate_e([img ; conv1(img)[c] ; conv2(img)[c] ; conv3(img)[c]])   each conv 1 -> C
+ *   x[q,:] = relu(bn2(fc(relu(bn1(y)) flattened channel-major)))
+ * `direction` does not enter: rel is indexed with r as given (rows num_rel/2.. of the reference's [2R, k] table
+ * are never read) and the head direction passes (t, r).  Pointers are device fp32 tensors with the reference's
+ * state_dict shapes: ent [N,200], rel [num_rel,200], bn0_* [1], conv1_weight [C,1,3,3], conv2/3_weight
+ * [C,C,3,3] (serial) or [C,1,3,3] (parallel), conv*_bias [C] — all three NULL for acre_bias = False, W_gate_e
+ * weight [400,1600] and bias [400] (parallel only; ignored by the serial way), bn1_* [C], fc_weight
+ * [200, C*400], fc_bias [200], bn2_* [200].
+ * x is [Q,200]; workspace >= kge_acre_trunk_workspace_bytes() bytes: per query the gate input (parallel only,
+ * C*1600 floats, 205 KB at C = 32), the features (C*400 floats, 51 KB at C = 32) and the Linear layer's slice
+ * partials (ceil(C*400/512)*200 floats); callers bound it by splitting Q.  Q = 0 is a no-op (e, r and x may
+ * then be NULL).
+ * KGE_EINVAL: way not 0 / 1, an atrous rate < 1, in_channels < 1, num_rel < 1, one or two (not zero or three)
+ * NULL conv biases, a NULL required pointer, or Q beyond one call's grid.  KGE_ENOTSUP: hidden_size != 200 (the
+ * reference's 10 x 20 view), a serial C whose maps and weight bank exceed 227 KB of shared memory
+ * (4*(400 + 800*C + 9*C*ceil8(C) + 3*ceil8(C)) bytes, so C <= 46), a parallel C whose image and banks exceed it
+ * (C <= 1923).  KGE_EWORKSPACE: a short workspace; nothing is written. */
+typedef struct kge_acre {
+  int32_t in_channels, way, first_atrous, second_atrous, third_atrous, hidden_size;
+  int64_t num_rel;
+  float bn0_eps, bn1_eps, bn2_eps;
+  const float* ent; const float* rel;
+  const float* bn0_weight; const float* bn0_bias; const float* bn0_mean; const float* bn0_var;
+  const float* conv1_weight; const float* conv1_bias;
+  const float* conv2_weight; const float* conv2_bias;
+  const float* conv3_weight; const float* conv3_bias;
+  const float* W_gate_e_weight; const float* W_gate_e_bias;
+  const float* bn1_weight; const float* bn1_bias; const float* bn1_mean; const float* bn1_var;
+  const float* fc_weight; const float* fc_bias;
+  const float* bn2_weight; const float* bn2_bias; const float* bn2_mean; const float* bn2_var;
+} kge_acre_t;
+int64_t kge_acre_trunk_workspace_bytes(const kge_acre_t* p, int64_t Q);
+int kge_acre_trunk_fwd(const kge_acre_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
+                       void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- negative sampling on the device: replaces the CPU sampler processes ----
  * process_function_pairwise / process_function_pointwise (pykg2vec/data/generator.py:42-158).

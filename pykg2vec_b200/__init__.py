@@ -40,6 +40,7 @@ MODEL_MAP = {
     "tucker": ("pykg2vec_b200.projection", "TuckER"),
     "hyper": ("pykg2vec_b200.projection", "HypER"),
     "interacte": ("pykg2vec_b200.projection", "InteractE"),
+    "acre": ("pykg2vec_b200.projection", "AcrE"),
 }
 
 

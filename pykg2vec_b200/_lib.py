@@ -11,7 +11,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_build", "libkge_b200.so")
 MAX_TABLES = 16
-ABI_VERSION = 7
+ABI_VERSION = 8
 ENOTSUP = -2   # include/kge_b200.h KGE_ENOTSUP
 
 MODEL_IDS = {
@@ -34,6 +34,7 @@ EXPORTS = [
     "kge_proj_tail_fwd", "kge_proj_tail_bwd", "kge_proj_bce", "kge_proj_rank_workspace_bytes", "kge_proj_rank", "kge_proj_labels",
     "kge_conve_trunk_workspace_bytes", "kge_conve_trunk_fwd", "kge_hyper_trunk_workspace_bytes", "kge_hyper_trunk_fwd",
     "kge_interacte_trunk_workspace_bytes", "kge_interacte_trunk_fwd",
+    "kge_acre_trunk_workspace_bytes", "kge_acre_trunk_fwd",
     "kge_project_entities", "kge_normalize_rows_to",
 ]
 
@@ -78,6 +79,7 @@ def lib():
     L.kge_conve_trunk_workspace_bytes.restype = ctypes.c_int64
     L.kge_hyper_trunk_workspace_bytes.restype = ctypes.c_int64
     L.kge_interacte_trunk_workspace_bytes.restype = ctypes.c_int64
+    L.kge_acre_trunk_workspace_bytes.restype = ctypes.c_int64
     if L.kge_abi_version() != ABI_VERSION:
         raise KgeError("libkge_b200.so ABI %d != binding ABI %d" % (L.kge_abi_version(), ABI_VERSION))
     _lib = L
@@ -660,6 +662,90 @@ def interacte_trunk_fwd(model, e, r, out=None, workspace=None, cap=None, perm=No
         check(lib().kge_interacte_trunk_fwd(ctypes.byref(p), _ptr(e[q0:q0 + n]), _ptr(r[q0:q0 + n]),
                                             ctypes.c_int64(n), _ptr(out[q0:q0 + n]), _ptr(workspace),
                                             ctypes.c_int64(workspace.numel()), _stream()), "kge_interacte_trunk_fwd")
+    return out
+
+
+ACRE_FIELDS = ("ent", "rel", "bn0_weight", "bn0_bias", "bn0_mean", "bn0_var", "conv1_weight", "conv1_bias",
+               "conv2_weight", "conv2_bias", "conv3_weight", "conv3_bias", "W_gate_e_weight", "W_gate_e_bias",
+               "bn1_weight", "bn1_bias", "bn1_mean", "bn1_var", "fc_weight", "fc_bias",
+               "bn2_weight", "bn2_bias", "bn2_mean", "bn2_var")
+ACRE_WAYS = {"serial": 0, "parallel": 1}
+# upper bound of the workspace one kge_acre_trunk_fwd call may use: per query the features take 51 KB at
+# in_channels 32 (serial) and the parallel way's W_gate_e input another 205 KB, so an Evaluator-sized batch is
+# split into chunks of queries (independent of each other: the result is the same bits as one call)
+ACRE_WORKSPACE_CAP = 256 << 20
+
+
+class KgeAcre(ctypes.Structure):
+    """kge_acre_t of include/kge_b200.h."""
+    _fields_ = [("in_channels", ctypes.c_int32), ("way", ctypes.c_int32), ("first_atrous", ctypes.c_int32),
+                ("second_atrous", ctypes.c_int32), ("third_atrous", ctypes.c_int32), ("hidden_size", ctypes.c_int32),
+                ("num_rel", ctypes.c_int64),
+                ("bn0_eps", ctypes.c_float), ("bn1_eps", ctypes.c_float), ("bn2_eps", ctypes.c_float)] + \
+        [(n, ctypes.c_void_p) for n in ACRE_FIELDS]
+
+
+def acre_struct(way, in_channels, atrous, hidden_size, num_rel):
+    """a KgeAcre holding the configuration only (pointers NULL).  way: "serial" / "parallel" (or 0 / 1; any other
+    value is passed on as -1 so that the call reports it); atrous: the three rates."""
+    p = KgeAcre()
+    p.way = ACRE_WAYS.get(way, way if way in (0, 1) else -1)
+    p.in_channels, p.hidden_size, p.num_rel = int(in_channels), int(hidden_size), int(num_rel)
+    p.first_atrous, p.second_atrous, p.third_atrous = (int(a) for a in atrous)
+    return p
+
+
+def acre_trunk_workspace_bytes(way, in_channels, atrous, hidden_size, num_rel, Q):
+    """bytes of device workspace ONE kge_acre_trunk_fwd call needs for Q queries (0 for an unsupported or
+    malformed configuration)"""
+    p = acre_struct(way, in_channels, atrous, hidden_size, num_rel)
+    return int(lib().kge_acre_trunk_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q)))
+
+
+def acre_trunk_fwd(model, e, r, out=None, workspace=None, cap=None):
+    """AcrE inference trunk (projection.py:706-734, eval mode): x [Q,200] for entity ids e and relation ids r
+    (both directions pass their own (entity, relation) pair: AcrE indexes rel_embeddings with r as given).
+    `model` is an AcrE with the reference's sub-module names.  The queries run in chunks whose workspace stays
+    under `cap` bytes (default ACRE_WORKSPACE_CAP; a single query always runs).  `workspace`: optional uint8
+    device buffer, grown if too small."""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    if r.numel() != Q:
+        raise KgeError("e and r must have equal length")
+    tensors = {"ent": model.ent_embeddings.weight, "rel": model.rel_embeddings.weight,
+               "fc_weight": model.fc.weight, "fc_bias": model.fc.bias}
+    for name in ("bn0", "bn1", "bn2"):
+        bn = getattr(model, name)
+        tensors.update({name + "_weight": bn.weight, name + "_bias": bn.bias,
+                        name + "_mean": bn.running_mean, name + "_var": bn.running_var})
+    for name in ("conv1", "conv2", "conv3"):
+        conv = getattr(model, name)
+        tensors.update({name + "_weight": conv.weight, name + "_bias": conv.bias})
+    gate = getattr(model, "W_gate_e", None)
+    if gate is not None:
+        tensors.update({"W_gate_e_weight": gate.weight, "W_gate_e_bias": gate.bias})
+    way = "serial" if model.way == "serial" else "parallel"      # the reference's test: any other value is parallel
+    p = acre_struct(way, model.in_channels, (model.first_atrous, model.second_atrous, model.third_atrous),
+                    model.ent_embeddings.weight.shape[1], model.rel_embeddings.weight.shape[0])
+    p.bn0_eps, p.bn1_eps, p.bn2_eps = float(model.bn0.eps), float(model.bn1.eps), float(model.bn2.eps)
+    for name in ACRE_FIELDS:
+        t = tensors.get(name)
+        setattr(p, name, None if t is None else _dev_f32(t.detach(), name).data_ptr())
+    if out is None:
+        out = torch.empty((Q, int(p.hidden_size)), dtype=torch.float32, device=e.device)
+    per_query = int(lib().kge_acre_trunk_workspace_bytes(ctypes.byref(p), ctypes.c_int64(1)))
+    if per_query == 0:    # unsupported configuration: the call below reports why
+        chunk = max(Q, 1)
+    else:
+        chunk = max(1, min(max(Q, 1), int(ACRE_WORKSPACE_CAP if cap is None else cap) // per_query))
+    nbytes = int(lib().kge_acre_trunk_workspace_bytes(ctypes.byref(p), ctypes.c_int64(chunk)))
+    if workspace is None or workspace.numel() < nbytes:
+        workspace = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=e.device)
+    for q0 in range(0, max(Q, 1), chunk):
+        n = min(chunk, Q - q0)
+        check(lib().kge_acre_trunk_fwd(ctypes.byref(p), _ptr(e[q0:q0 + n]), _ptr(r[q0:q0 + n]), ctypes.c_int64(n),
+                                       _ptr(out[q0:q0 + n]), _ptr(workspace), ctypes.c_int64(workspace.numel()),
+                                       _stream()), "kge_acre_trunk_fwd")
     return out
 
 

@@ -1,9 +1,10 @@
 // kge_proj.cu — C-ABI launchers of the projection-model tail (kernels and launch plans:
-// kge_proj.cuh) and of the ConvE, HypER and InteractE inference trunks (kge_conve.cuh, kge_hyper.cuh,
-// kge_interacte.cuh, which reuse the same tiled GEMM — one translation unit so the kernel template is
-// instantiated once).  Declarations and reference citations: include/kge_b200.h.
+// kge_proj.cuh) and of the ConvE, HypER, InteractE and AcrE inference trunks (kge_conve.cuh, kge_hyper.cuh,
+// kge_interacte.cuh, kge_acre.cuh, which reuse the same tiled GEMM — one translation unit so the kernel
+// template is instantiated once).  Declarations and reference citations: include/kge_b200.h.
 #include <cstdlib>
 
+#include "kge_acre.cuh"
 #include "kge_interacte.cuh"
 
 using namespace kge;
@@ -330,6 +331,119 @@ int kge_interacte_trunk_fwd(const kge_interacte_t* p, const int64_t* e, const in
   hyper_fc_combine_kernel<<<proj_tiles(Q * k, 256), 256, 0, st>>>(partial, conve_fc_slices(Fw), Q * k, k, p->fc_bias,
                                                                   p->bn2_weight, p->bn2_bias, p->bn2_mean,
                                                                   p->bn2_var, p->bn2_eps, x);
+  KGE_CHECK_LAUNCH("hyper_fc_combine_kernel");
+  return KGE_OK;
+}
+
+
+// ---- AcrE inference trunk -----------------------------------------------------------------
+
+// KGE_OK, or the error code of an unsupported / malformed configuration (message set for `fn`)
+static int acre_shape(const kge_acre_t* p, const char* fn) {
+  const int C = p->in_channels;
+  if ((p->way != 0 && p->way != 1) || C < 1 || p->first_atrous < 1 || p->second_atrous < 1 ||
+      p->third_atrous < 1 || p->num_rel < 1) {
+    set_error("%s: bad configuration way=%d in_channels=%d atrous %d/%d/%d num_rel %lld", fn, p->way, C,
+              p->first_atrous, p->second_atrous, p->third_atrous, (long long)p->num_rel);
+    return KGE_EINVAL;
+  }
+  if (p->hidden_size != ACRE_K) {
+    set_error("%s: unsupported hidden_size %d (the trunk views each row as 10 x 20: needs 200)", fn,
+              p->hidden_size);
+    return KGE_ENOTSUP;
+  }
+  const long long smem = (p->way == 0 ? acre_serial_smem(C).total : acre_gate_smem(C)) * (long long)sizeof(float);
+  if (smem > ACRE_SMEM_MAX) {
+    set_error("%s: in_channels %d needs %lld bytes of shared memory in the %s way (max %d)", fn, C, smem,
+              p->way == 0 ? "serial" : "parallel", ACRE_SMEM_MAX);
+    return KGE_ENOTSUP;
+  }
+  return KGE_OK;
+}
+
+int64_t kge_acre_trunk_workspace_bytes(const kge_acre_t* p, int64_t Q) {
+  if (!p || acre_shape(p, "kge_acre_trunk_workspace_bytes")) return 0;
+  return acre_layout(Q > 0 ? Q : 1, p->in_channels, p->way == 1).total * (int64_t)sizeof(float);
+}
+
+int kge_acre_trunk_fwd(const kge_acre_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
+                       void* workspace, int64_t workspace_bytes, void* stream) {
+  if (!p || !workspace || (Q > 0 && (!e || !r || !x))) {   // an empty batch may pass null id / output pointers
+    set_error("kge_acre_trunk_fwd: null pointer");
+    return KGE_EINVAL;
+  }
+  if (int rc = acre_shape(p, "kge_acre_trunk_fwd")) return rc;
+  const bool par = p->way == 1;
+  const float* ptrs[] = {p->ent, p->rel, p->bn0_weight, p->bn0_bias, p->bn0_mean, p->bn0_var, p->conv1_weight,
+                         p->conv2_weight, p->conv3_weight, p->bn1_weight, p->bn1_bias, p->bn1_mean, p->bn1_var,
+                         p->fc_weight, p->fc_bias, p->bn2_weight, p->bn2_bias, p->bn2_mean, p->bn2_var};
+  for (const float* t : ptrs)
+    if (!t) { set_error("kge_acre_trunk_fwd: null parameter tensor"); return KGE_EINVAL; }
+  if (par && (!p->W_gate_e_weight || !p->W_gate_e_bias)) {
+    set_error("kge_acre_trunk_fwd: the parallel way needs W_gate_e");
+    return KGE_EINVAL;
+  }
+  const int nbias = (p->conv1_bias != nullptr) + (p->conv2_bias != nullptr) + (p->conv3_bias != nullptr);
+  if (nbias != 0 && nbias != 3) {
+    set_error("kge_acre_trunk_fwd: conv biases must be all set (acre_bias) or all NULL");
+    return KGE_EINVAL;
+  }
+  const int C = p->in_channels;
+  if (Q < 0 || (Q + PBM - 1) / PBM > 65535 || (par && (Q * C + PBM - 1) / PBM > 65535)) {
+    set_error("kge_acre_trunk_fwd: bad Q %lld for in_channels %d", (long long)Q, C);
+    return KGE_EINVAL;
+  }
+  if (workspace_bytes < kge_acre_trunk_workspace_bytes(p, Q)) {
+    set_error("kge_acre_trunk_fwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  if (Q == 0) return KGE_OK;
+  cudaStream_t st = (cudaStream_t)stream;
+  const AcreLayout lay = acre_layout(Q, C, par);
+  float* ws = (float*)workspace;
+  AcreFeat f{};
+  f.ent = p->ent; f.rel = p->rel; f.e = e; f.r = r; f.C = C;
+  f.dil[0] = p->first_atrous; f.dil[1] = p->second_atrous; f.dil[2] = p->third_atrous;
+  f.bn0_w = p->bn0_weight; f.bn0_b = p->bn0_bias; f.bn0_mean = p->bn0_mean; f.bn0_var = p->bn0_var;
+  f.bn0_eps = p->bn0_eps;
+  f.conv_w[0] = p->conv1_weight; f.conv_w[1] = p->conv2_weight; f.conv_w[2] = p->conv3_weight;
+  f.conv_b[0] = p->conv1_bias; f.conv_b[1] = p->conv2_bias; f.conv_b[2] = p->conv3_bias;
+  f.bn1_w = p->bn1_weight; f.bn1_b = p->bn1_bias; f.bn1_mean = p->bn1_mean; f.bn1_var = p->bn1_var;
+  f.bn1_eps = p->bn1_eps;
+  float* feat = ws + lay.feat;
+  if (!par) {
+    f.out = feat;
+    const size_t smem = (size_t)acre_serial_smem(C).total * sizeof(float);
+    if (smem > 48 * 1024)
+      KGE_CUDA_OK(cudaFuncSetAttribute(acre_serial_feature_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)smem));
+    acre_serial_feature_kernel<<<(unsigned)Q, ACRE_THREADS, smem, st>>>(f);
+    KGE_CHECK_LAUNCH("acre_serial_feature_kernel");
+  } else {
+    f.out = ws + lay.gate;
+    const size_t smem = (size_t)acre_gate_smem(C) * sizeof(float);
+    if (smem > 48 * 1024)
+      KGE_CUDA_OK(cudaFuncSetAttribute(acre_gate_input_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                       (int)smem));
+    acre_gate_input_kernel<<<(unsigned)Q, ACRE_GATE_THREADS, smem, st>>>(f);
+    KGE_CHECK_LAUNCH("acre_gate_input_kernel");
+    const long long rows = Q * C;
+    if (int rc = launch_gemm<EPI_STORE>(acre_plan_gate(f.out, p->W_gate_e_weight, p->W_gate_e_bias, rows, feat,
+                                                       pick_tile(rows, ACRE_PIX)), st, "proj_gemm_kernel<acre gate>"))
+      return rc;
+    acre_bn1_relu_kernel<<<proj_tiles(rows * ACRE_PIX, 256), 256, 0, st>>>(feat, rows * ACRE_PIX, C, p->bn1_weight,
+                                                                          p->bn1_bias, p->bn1_mean, p->bn1_var,
+                                                                          p->bn1_eps);
+    KGE_CHECK_LAUNCH("acre_bn1_relu_kernel");
+  }
+  const long long Fw = acre_feat_width(C);
+  float* partial = ws + lay.partial;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_fc(feat, p->fc_weight, Q, Fw, ACRE_K, partial), st,
+                                      "proj_gemm_kernel<acre fc>")) return rc;
+  hyper_fc_combine_kernel<<<proj_tiles(Q * ACRE_K, 256), 256, 0, st>>>(partial, conve_fc_slices(Fw), Q * ACRE_K,
+                                                                      ACRE_K, p->fc_bias, p->bn2_weight,
+                                                                      p->bn2_bias, p->bn2_mean, p->bn2_var,
+                                                                      p->bn2_eps, x);
   KGE_CHECK_LAUNCH("hyper_fc_combine_kernel");
   return KGE_OK;
 }

@@ -26,6 +26,13 @@ InteractE (projection.py:347-505) has the same tail and loss; its trunk stacks P
 entity and relation features and convolves them circularly with one shared filter bank.  Training runs the
 reference's layers; evaluation without autograd runs kge_interacte_trunk_fwd — one kernel for gather +
 permutation + bn0 + circular conv + bn1 + ReLU, then HypER's Linear GEMM and bn2 + ReLU.
+
+AcrE (projection.py:621-746) has the same tail and loss; its trunk runs three dilated (atrous) 3x3 convolutions
+on the 20 x 20 image of the stacked entity and relation rows, chained with a residual add (serial way) or side
+by side and mixed per channel by a Linear gate (parallel way).  Training runs the reference's layers;
+evaluation without autograd runs kge_acre_trunk_fwd — one kernel for gather + bn0 + the three convs (+ residual
++ bn1 + ReLU in the serial way; the gate input in the parallel way, then the gate on the tiled GEMM and bn1 +
+ReLU), then HypER's Linear GEMM and bn2 + ReLU.
 """
 import numpy as np
 import torch
@@ -405,6 +412,110 @@ class HypER(ProjectionModel):
 
     def forward(self, e, r, direction="tail"):
         return ProjTailFunction.apply(self.proj_query(e, r, direction), self.ent_embeddings.weight, self.b)
+
+    def predict_tail_rank(self, e, r, topk=-1):
+        _, rank = torch.topk(-self.forward(e, r, direction="tail"), k=topk)
+        return rank
+
+    def predict_head_rank(self, e, r, topk=-1):
+        _, rank = torch.topk(-self.forward(e, r, direction="head"), k=topk)
+        return rank
+
+
+class AcrE(ProjectionModel):
+    """pykg2vec/models/projection.py:621-746 — same kwargs, sub-module names and state_dict keys and order (bias /
+    ent_embeddings / rel_embeddings / bn0 / bn1 / bn2 / fc / conv1 / conv2 / conv3, then W_gate_e in the parallel
+    way), parameter_list and loss binding.  rel_embeddings has 2 * tot_relation rows, but as in the reference
+    `direction` is validated and otherwise ignored: both directions index it with r as given (rows R..2R-1 are
+    never read) and the head direction runs the same function on (t, r).  The trunk views each 200-wide row as
+    10 x 20, so hidden_size must be 200 for the reference's forward to mean anything; the class constructs for
+    any size, as upstream, and the evaluation kernel refuses the others (KgeNotSupported).
+
+    Training runs the reference's layers (the three convolutions through _Fp32Conv2d with their dilation and
+    padding, TF32 off); evaluation without autograd runs kge_acre_trunk_fwd."""
+
+    def __init__(self, **kwargs):
+        super(AcrE, self).__init__(self.__class__.__name__.lower())
+        param_list = ["tot_entity", "tot_relation", "hidden_size", "input_dropout", "hidden_dropout",
+                      "feature_map_dropout", "in_channels", "way", "first_atrous", "second_atrous", "third_atrous",
+                      "acre_bias"]
+        param_dict = self.load_params(param_list, kwargs)
+        self.__dict__.update(param_dict)
+        k, C = self.hidden_size, self.in_channels
+        # construction order = the reference's: it fixes the state_dict order and the torch draws
+        self.ent_embeddings = NamedEmbedding("ent_embedding", self.tot_entity, k, padding_idx=None)
+        self.rel_embeddings = NamedEmbedding("rel_embedding", self.tot_relation * 2, k, padding_idx=None)
+        self.inp_drop = nn.Dropout(self.input_dropout)
+        self.hidden_drop = nn.Dropout(self.hidden_dropout)
+        self.feature_map_drop = nn.Dropout2d(self.feature_map_dropout)
+        self.bn0 = nn.BatchNorm2d(1)
+        self.bn1 = nn.BatchNorm2d(C)
+        self.bn2 = nn.BatchNorm1d(k)
+        self.fc = nn.Linear(C * 400, k)
+        self.padding = 0
+        # conv l: 3x3, stride 1, padding = dilation = its atrous rate; serial: 1 -> C -> C -> C, else three 1 -> C
+        cin = C if self.way == "serial" else 1
+        self.conv1 = nn.Conv2d(1, C, (3, 3), 1, self.first_atrous, bias=self.acre_bias, dilation=self.first_atrous)
+        self.conv2 = nn.Conv2d(cin, C, (3, 3), 1, self.second_atrous, bias=self.acre_bias,
+                               dilation=self.second_atrous)
+        self.conv3 = nn.Conv2d(cin, C, (3, 3), 1, self.third_atrous, bias=self.acre_bias, dilation=self.third_atrous)
+        if self.way != "serial":
+            self.W_gate_e = nn.Linear(1600, 400)
+        self.register_parameter("bias", nn.Parameter(torch.zeros(self.tot_entity)))
+        nn.init.xavier_uniform_(self.ent_embeddings.weight.data)
+        nn.init.xavier_uniform_(self.rel_embeddings.weight.data)
+        self.parameter_list = [self.ent_embeddings, self.rel_embeddings]
+        self.loss = Criterion.multi_class_bce
+
+    def embed(self, h, r, t):
+        return self.ent_embeddings(h), self.rel_embeddings(r), self.ent_embeddings(t)
+
+    def embed2(self, e, r):
+        return self.ent_embeddings(e), self.rel_embeddings(r)
+
+    # ---- trunk: AcrE.forward before the x . E^T product (projection.py:708-734) ----
+    def _trunk_layers(self, e, r):
+        emb_e, emb_r = self.embed2(e, r)
+        x = torch.cat([emb_e.view(-1, 1, 10, 20), emb_r.view(-1, 1, 10, 20)], dim=2)
+        x = self.bn0(x)
+        x = self.inp_drop(x)
+        res = x
+        C = self.in_channels
+        if self.way == "serial":
+            x = _conv2d_fp32(self.conv1, x)
+            x = _conv2d_fp32(self.conv2, x)
+            x = _conv2d_fp32(self.conv3, x)
+            x = x + res
+        else:
+            conv1 = _conv2d_fp32(self.conv1, x).view(-1, C, 400)
+            conv2 = _conv2d_fp32(self.conv2, x).view(-1, C, 400)
+            conv3 = _conv2d_fp32(self.conv3, x).view(-1, C, 400)
+            res = res.expand(-1, C, 20, 20).view(-1, C, 400)
+            x = torch.cat((res, conv1, conv2, conv3), dim=2)
+            x = self.W_gate_e(x).view(-1, C, 20, 20)
+        x = self.bn1(x)
+        x = torch.relu(x)
+        x = self.feature_map_drop(x)
+        x = x.view(x.shape[0], -1)
+        x = self.fc(x)
+        x = self.hidden_drop(x)
+        x = self.bn2(x)   # applied in both modes (unlike ConvE)
+        return torch.relu(x)
+
+    def proj_query(self, e, r, direction="tail"):
+        """x [b, k]: the operand of the tail product, for the batched Evaluator (eval mode)."""
+        assert direction in ("head", "tail"), "Unknown forward direction"
+        _require_cuda(e, r, self.ent_embeddings.weight)
+        if not self.training and not torch.is_grad_enabled():
+            return _lib.acre_trunk_fwd(self, e.contiguous(), r.contiguous())
+        return self._trunk_layers(e, r)
+
+    def proj_tail_tables(self):
+        """(entity table [N,k], bias row [N]) of the tail product."""
+        return self.ent_embeddings.weight, self.bias
+
+    def forward(self, e, r, direction="tail"):
+        return ProjTailFunction.apply(self.proj_query(e, r, direction), self.ent_embeddings.weight, self.bias)
 
     def predict_tail_rank(self, e, r, topk=-1):
         _, rank = torch.topk(-self.forward(e, r, direction="tail"), k=topk)
