@@ -135,18 +135,11 @@ KGE_DEV void dist_elem(const DistCtx& X, float hv, float rv, float tv, float& dh
   dt = -(dx - tn * X.ct) * X.it;
 }
 
-// TransE / TransM backward with the three rows held in registers (CH chunks per lane):
-// one trip to memory for the operands, then norms, projections and the scatter from registers.
+// TransE / TransM backward with the three rows held in registers (CH chunks per lane, as load_trans_chunks
+// fills them): norms, projections and the scatter from registers.
 template <int CH, int VEC>
-KGE_DEV void grad_trans_cached(const TripleRows& R, const GradRows& G, int d, int nch, int lane, int l1,
-                               float gs) {
-  float4 A[CH], B[CH], C[CH];
-#pragma unroll
-  for (int k = 0; k < CH; ++k) {
-    const int c = lane + 8 * k;
-    if (c < nch) { A[k] = ld_chunk<VEC>(R.h[0], c, d); B[k] = ld_chunk<VEC>(R.r[0], c, d); C[k] = ld_chunk<VEC>(R.t[0], c, d); }
-    else { A[k] = B[k] = C[k] = make_float4(0.f, 0.f, 0.f, 0.f); }
-  }
+KGE_DEV void grad_trans_regs(const float4 (&A)[CH], const float4 (&B)[CH], const float4 (&C)[CH], const GradRows& G,
+                             int d, int nch, int lane, int l1, float gs) {
   DistCtx X;
   float sh = 0.f, sr = 0.f, st = 0.f;
 #pragma unroll
@@ -190,6 +183,17 @@ KGE_DEV void grad_trans_cached(const TripleRows& R, const GradRows& G, int d, in
       red_row_chunk<VEC>(G.t[0], c, d, dt);
     }
   }
+}
+
+// ... with one trip to memory for the operands
+template <int CH, int VEC>
+KGE_DEV void grad_trans_cached(const TripleRows& R, const GradRows& G, int d, int nch, int lane, int l1,
+                               float gs) {
+  float4 A[CH], B[CH], C[CH];
+  load_trans_chunks<CH>([&](int c) { return ld_chunk<VEC>(R.h[0], c, d); },
+                        [&](int c) { return ld_chunk<VEC>(R.r[0], c, d); },
+                        [&](int c) { return ld_chunk<VEC>(R.t[0], c, d); }, nch, lane, A, B, C);
+  grad_trans_regs<CH, VEC>(A, B, C, G, d, nch, lane, l1, gs);
 }
 
 // Accumulate gs * d score / d rows into G.  All 8 lanes call; `scratch` per group

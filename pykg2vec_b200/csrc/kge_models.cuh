@@ -181,64 +181,80 @@ KGE_DEV void hyper_product(const float* hc, float* rc /* in: raw, out: normalise
 // Shared tail of TransE/H/D/R/M forward(): L2-normalise h', r', t' and return
 // ||h^ + r^ - t^||_p  (pairwise.py:69-76, :146-153, :266-273, :463-470).
 // fh/fr/ft(c) return chunk c (4 elements, zero beyond the width) of each operand.
-// CH > 0: the lane's chunks (c = lane + 8k, k < CH) are fetched ONCE into registers and both
-// passes (norms, then distance) run from registers — one trip to memory instead of two.
-template <int GROUPING, int CH, class FH, class FR, class FT>
-KGE_DEV float trans_distance_impl(FH fh, FR fr, FT ft, int nch, int lane, int l1) {
-  float4 A[CH > 0 ? CH : 1], B[CH > 0 ? CH : 1], C[CH > 0 ? CH : 1];
-  if (CH > 0) {
+// CH > 0: the lane's chunks (c = lane + 8k, k < CH) are fetched ONCE into registers (load_trans_chunks) and
+// both passes (norms, then distance) run from registers (trans_distance_regs) — one trip to memory instead of two.
+template <int GROUPING>
+KGE_DEV void trans_distance_step(const float4& a, const float4& b, const float4& cc, float ih, float ir, float it,
+                                 int l1, float& acc) {
 #pragma unroll
-    for (int k = 0; k < CH; ++k) {
-      const int c = lane + 8 * k;
-      if (c < nch) { A[k] = fh(c); B[k] = fr(c); C[k] = ft(c); }
-      else { A[k] = B[k] = C[k] = make_float4(0.f, 0.f, 0.f, 0.f); }
-    }
+  for (int e = 0; e < 4; ++e) {
+    const float hn = fmul(f4_get(a, e), ih), rn = fmul(f4_get(b, e), ir), tn = fmul(f4_get(cc, e), it);
+    float x;
+    if (GROUPING == KGE_GROUP_TAIL) x = fsub(fadd(hn, rn), tn);
+    else x = fadd(hn, fsub(rn, tn));
+    if (l1) acc = fadd(acc, fabsf(x)); else acc = ffma(x, x, acc);
   }
+}
+
+template <int CH, class FH, class FR, class FT>
+KGE_DEV void load_trans_chunks(FH fh, FR fr, FT ft, int nch, int lane, float4 (&A)[CH], float4 (&B)[CH],
+                               float4 (&C)[CH]) {
+#pragma unroll
+  for (int k = 0; k < CH; ++k) {
+    const int c = lane + 8 * k;
+    if (c < nch) { A[k] = fh(c); B[k] = fr(c); C[k] = ft(c); }
+    else { A[k] = B[k] = C[k] = make_float4(0.f, 0.f, 0.f, 0.f); }
+  }
+}
+
+template <int GROUPING, int CH>
+KGE_DEV float trans_distance_regs(const float4 (&A)[CH], const float4 (&B)[CH], const float4 (&C)[CH], int l1) {
   float sh = 0.f, sr = 0.f, st = 0.f;
-  if (CH > 0) {
 #pragma unroll
-    for (int k = 0; k < CH; ++k) {
+  for (int k = 0; k < CH; ++k) {
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        sh = ffma(f4_get(A[k], e), f4_get(A[k], e), sh);
-        sr = ffma(f4_get(B[k], e), f4_get(B[k], e), sr);
-        st = ffma(f4_get(C[k], e), f4_get(C[k], e), st);
-      }
-    }
-  } else {
-#pragma unroll 2
-    for (int c = lane; c < nch; c += 8) {
-      const float4 a = fh(c), b = fr(c), cc = ft(c);
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        sh = ffma(f4_get(a, e), f4_get(a, e), sh);
-        sr = ffma(f4_get(b, e), f4_get(b, e), sr);
-        st = ffma(f4_get(cc, e), f4_get(cc, e), st);
-      }
+    for (int e = 0; e < 4; ++e) {
+      sh = ffma(f4_get(A[k], e), f4_get(A[k], e), sh);
+      sr = ffma(f4_get(B[k], e), f4_get(B[k], e), sr);
+      st = ffma(f4_get(C[k], e), f4_get(C[k], e), st);
     }
   }
   const float ih = inv_norm_from_sumsq(group_sum(sh));
   const float ir = inv_norm_from_sumsq(group_sum(sr));
   const float it = inv_norm_from_sumsq(group_sum(st));
   float acc = 0.f;
-  auto step = [&](const float4& a, const float4& b, const float4& cc) {
+  // zero-filled slots beyond the row add exact zeros: same bits as skipping them
+#pragma unroll
+  for (int k = 0; k < CH; ++k) trans_distance_step<GROUPING>(A[k], B[k], C[k], ih, ir, it, l1, acc);
+  acc = group_sum(acc);
+  return l1 ? acc : __fsqrt_rn(acc);
+}
+
+template <int GROUPING, int CH, class FH, class FR, class FT>
+KGE_DEV float trans_distance_impl(FH fh, FR fr, FT ft, int nch, int lane, int l1) {
+  if (CH > 0) {
+    constexpr int K = CH > 0 ? CH : 1;
+    float4 A[K], B[K], C[K];
+    load_trans_chunks<K>(fh, fr, ft, nch, lane, A, B, C);
+    return trans_distance_regs<GROUPING, K>(A, B, C, l1);
+  }
+  float sh = 0.f, sr = 0.f, st = 0.f;
+#pragma unroll 2
+  for (int c = lane; c < nch; c += 8) {
+    const float4 a = fh(c), b = fr(c), cc = ft(c);
 #pragma unroll
     for (int e = 0; e < 4; ++e) {
-      const float hn = fmul(f4_get(a, e), ih), rn = fmul(f4_get(b, e), ir), tn = fmul(f4_get(cc, e), it);
-      float x;
-      if (GROUPING == KGE_GROUP_TAIL) x = fsub(fadd(hn, rn), tn);
-      else x = fadd(hn, fsub(rn, tn));
-      if (l1) acc = fadd(acc, fabsf(x)); else acc = ffma(x, x, acc);
+      sh = ffma(f4_get(a, e), f4_get(a, e), sh);
+      sr = ffma(f4_get(b, e), f4_get(b, e), sr);
+      st = ffma(f4_get(cc, e), f4_get(cc, e), st);
     }
-  };
-  if (CH > 0) {
-    // zero-filled slots beyond the row add exact zeros: same bits as skipping them
-#pragma unroll
-    for (int k = 0; k < CH; ++k) step(A[k], B[k], C[k]);
-  } else {
-#pragma unroll 2
-    for (int c = lane; c < nch; c += 8) step(fh(c), fr(c), ft(c));
   }
+  const float ih = inv_norm_from_sumsq(group_sum(sh));
+  const float ir = inv_norm_from_sumsq(group_sum(sr));
+  const float it = inv_norm_from_sumsq(group_sum(st));
+  float acc = 0.f;
+#pragma unroll 2
+  for (int c = lane; c < nch; c += 8) trans_distance_step<GROUPING>(fh(c), fr(c), ft(c), ih, ir, it, l1, acc);
   acc = group_sum(acc);
   return l1 ? acc : __fsqrt_rn(acc);
 }

@@ -4,10 +4,10 @@
 // loss.backward() (:298) and optimizer.step() (:299) for optim.SGD / optim.Adagrad
 // over dense nn.Embedding gradients.
 //
-//   kernel A (train_hinge_kernel): one 8-lane group per (positive, negative) pair:
-//     both scores (canonical arithmetic, == forward()), hinge term, and for active
-//     pairs the row gradients of both triples scattered into a zero-filled dense
-//     gradient scratch G.
+//   kernel A (train_hinge_kernel): one 8-lane group per triple, the positive's and the negative's groups of
+//     a pair side by side in one warp: both scores (canonical arithmetic, == forward()), the hinge term from
+//     one shuffle, and for active pairs each group scatters its triple's row gradients into a zero-filled
+//     dense gradient scratch G.
 //   kernel B (apply_rows_kernel): for every (table, id) the batch touched, take the
 //     accumulated row gradient out of G with atomicExch(.,0) — duplicates of a row see
 //     zeros — and apply the optimizer to that row.  G is zero again afterwards, and
@@ -22,52 +22,74 @@ constexpr int kGroupsPerCta = kThreads / 8;
 
 struct GradTablesT { float* t[KGE_MAX_TABLES]; };
 
-template <int MODEL, int VEC>
-__global__ void __launch_bounds__(kThreads)
+// A training batch is a few hundred pairs of pure latency: small CTAs (4 pairs) spread B = 512 over 128 SMs.
+constexpr int kHingeThreads = 64;
+constexpr int kHingeGroups = kHingeThreads / 8;
+
+// CH > 0 (TransE / TransM, 16-byte rows, ch_select(d) = CH): the triple's three rows are read once into
+// registers and both the score and the gradient are computed from them.  CH = 0: the looped (not register-cached)
+// forms of the score / gradient functions — with both triples of a pair cached in one group this kernel was
+// 12,760 instructions and stalled on instruction fetch.  Every form has the same arithmetic order, same bits.
+constexpr int hinge_ch(int model, int vec, int ch) {
+  return (model == KGE_TRANSE || model == KGE_TRANSM) && vec == 4 ? ch : 0;
+}
+
+template <int MODEL, int VEC, int CH>
+__global__ void __launch_bounds__(kHingeThreads)
 train_hinge_kernel(ModelParams P, GradTablesT GT, const int64_t* __restrict__ ph,
                    const int64_t* __restrict__ pr, const int64_t* __restrict__ pt,
                    const int64_t* __restrict__ nh, const int64_t* __restrict__ nr,
                    const int64_t* __restrict__ nt, int64_t n, float margin,
                    float* __restrict__ loss, int scratch_floats) {
   extern __shared__ float4 smem_f4[];
-  __shared__ float red[kThreads / 32];
+  __shared__ float red[kHingeThreads / 32];
   float* scratch = reinterpret_cast<float*>(smem_f4) + (size_t)(threadIdx.x >> 3) * scratch_floats;
   const int lane = threadIdx.x & 7;
-  const int64_t g = (int64_t)blockIdx.x * kGroupsPerCta + (threadIdx.x >> 3);
-  float v = 0.f;
-  if (g < n) {
-    const int64_t a = __ldg(ph + g), b = __ldg(pr + g), c = __ldg(pt + g);
-    const int64_t x = __ldg(nh + g), y = __ldg(nr + g), z = __ldg(nt + g);
-    TripleRows Rp, Rn;
-    resolve_rows<MODEL>(Rp, P, P.tab, P.tab, P.tab, a, b, c);
-    resolve_rows<MODEL>(Rn, P, P.tab, P.tab, P.tab, x, y, z);
-    prefetch_triple_rows(Rp, P.d, P.dr, lane);   // all six rows' cold misses overlap (the phases below are dependent)
-    prefetch_triple_rows(Rn, P.d, P.dr, lane);
-    // CHSEL = 0: the looped (not register-cached, not unrolled-by-width) forms of the score / gradient
-    // functions.  A training batch is a few hundred groups — pure latency —, and the cached forms made this
-    // kernel 12,760 instructions (204 KB) and stalled it on instruction fetch.  Same arithmetic order, same bits.
-    const float sp = score_group<MODEL, VEC, KGE_GROUP_TAIL, 0>(Rp, P, lane, scratch);
-    const float sn = score_group<MODEL, VEC, KGE_GROUP_TAIL, 0>(Rn, P, lane, scratch);
-    v = fmaxf(fsub(fadd(sp, margin), sn), 0.f);  // Criterion.pairwise_hinge, criterion.py:26-29
-    if (v > 0.f) {
-      GradRows Gp, Gn;
-      resolve_grad_rows<MODEL>(Gp, P, GT.t, a, b, c);
-      resolve_grad_rows<MODEL>(Gn, P, GT.t, x, y, z);
-      grad_group<MODEL, VEC, 0>(Rp, Gp, P, lane, 1.f, scratch);
-      grad_group<MODEL, VEC, 0>(Rn, Gn, P, lane, -1.f, scratch);
+  const bool neg = (threadIdx.x >> 3) & 1;                  // group 2k: the positive, 2k + 1: its negative
+  const int64_t g = (int64_t)blockIdx.x * (kHingeGroups / 2) + (threadIdx.x >> 4);
+  const bool valid = g < n;                                 // (the same for both groups of a pair)
+  int64_t a = 0, b = 0, c = 0;
+  TripleRows R;
+  float s = 0.f;
+  constexpr int K = CH > 0 ? CH : 1;
+  float4 A[K], Bv[K], C[K];
+  if (valid) {
+    a = __ldg((neg ? nh : ph) + g); b = __ldg((neg ? nr : pr) + g); c = __ldg((neg ? nt : pt) + g);
+    resolve_rows<MODEL>(R, P, P.tab, P.tab, P.tab, a, b, c);
+    if (CH > 0) {
+      const int d = P.d, nch = (d + 3) >> 2;
+      load_trans_chunks<K>([&](int q) { return ld_chunk<VEC>(R.h[0], q, d); },
+                           [&](int q) { return ld_chunk<VEC>(R.r[0], q, d); },
+                           [&](int q) { return ld_chunk<VEC>(R.t[0], q, d); }, nch, lane, A, Bv, C);
+      s = trans_distance_regs<KGE_GROUP_TAIL, K>(A, Bv, C, P.l1);
+      if (MODEL == KGE_TRANSM) s = fmul(__ldg(R.r[1]), s);   // == score_group
+    } else {
+      prefetch_triple_rows(R, P.d, P.dr, lane);   // the row misses of the dependent phases below overlap
+      s = score_group<MODEL, VEC, KGE_GROUP_TAIL, 0>(R, P, lane, scratch);
     }
-    if (lane != 0) v = 0.f;
   }
+  const float so = __shfl_xor_sync(0xffffffffu, s, 8);      // the other triple of the pair
+  const float sp = neg ? so : s, sn = neg ? s : so;
+  float v = fmaxf(fsub(fadd(sp, margin), sn), 0.f);        // Criterion.pairwise_hinge, criterion.py:26-29
+  if (valid && v > 0.f) {
+    GradRows G;
+    resolve_grad_rows<MODEL>(G, P, GT.t, a, b, c);
+    const float gs = neg ? -1.f : 1.f;
+    if (CH > 0) grad_trans_regs<K, VEC>(A, Bv, C, G, P.d, (P.d + 3) >> 2, lane, P.l1,
+                                        MODEL == KGE_TRANSM ? gs * __ldg(R.r[1]) : gs);   // == grad_group
+    else grad_group<MODEL, VEC, 0>(R, G, P, lane, gs, scratch);
+  }
+  if (!valid || neg || lane != 0) v = 0.f;
   // batch loss: block tree + one atomic per CTA
 #pragma unroll
   for (int off = 16; off; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
   if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
   __syncthreads();
   if (threadIdx.x == 0) {
-    float s = 0.f;
+    float t = 0.f;
 #pragma unroll
-    for (int w = 0; w < kThreads / 32; ++w) s += red[w];
-    if (s != 0.f) atomicAdd(loss, s);
+    for (int w = 0; w < kHingeThreads / 32; ++w) t += red[w];
+    if (t != 0.f) atomicAdd(loss, t);
   }
 }
 
@@ -244,12 +266,19 @@ KGE_DEV float apply_elem(float wv, float gv, float* s, float lr, float eps) {
   return fsub(wv, fmul(lr, __fdiv_rn(gv, fadd(__fsqrt_rn(sv), eps))));
 }
 
+// One 8-lane group per (task, row); 8 rows per CTA, so that the 3,072 rows of a B = 512 TransE step spread over
+// every SM.  A lane's chunks of a 16-byte-aligned row go in three round trips per 8 chunks (rows up to 256 floats
+// in one pass): all atomic exchanges, then the weights (and state) of the nonzero chunks, then the stores.
+constexpr int kApplyThreads = 64;
+constexpr int kApplyGroups = kApplyThreads / 8;
+constexpr int kApplyChunks = 8;
+
 template <int OPT>
-__global__ void __launch_bounds__(kThreads)
+__global__ void __launch_bounds__(kApplyThreads)
 apply_rows_kernel(ApplyTasks T, int64_t n, float lr, float eps) {
   const int task = blockIdx.y;
   const int lane = threadIdx.x & 7;
-  const int64_t i = (int64_t)blockIdx.x * kGroupsPerCta + (threadIdx.x >> 3);
+  const int64_t i = (int64_t)blockIdx.x * kApplyGroups + (threadIdx.x >> 3);
   if (i >= n) return;
   const int width = T.width[task];
   const size_t off = (size_t)__ldg(T.ids[task] + i) * (size_t)width;
@@ -259,17 +288,34 @@ apply_rows_kernel(ApplyTasks T, int64_t n, float lr, float eps) {
   const bool vec = ((width & 3) == 0) && ((((uintptr_t)w | (uintptr_t)g | (uintptr_t)(OPT == 1 ? s : w)) & 15) == 0);
   if (vec) {
     const int nch = width >> 2;
-    for (int c = lane; c < nch; c += 8) {
-      const float4 gv = exch_zero_b128(g + 4 * c);
-      if (gv.x != 0.f || gv.y != 0.f || gv.z != 0.f || gv.w != 0.f) {
-        float4 wv = *reinterpret_cast<float4*>(w + 4 * c);
-        float4 sv = (OPT == 1) ? *reinterpret_cast<float4*>(s + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
-        wv.x = apply_elem<OPT>(wv.x, gv.x, &sv.x, lr, eps);
-        wv.y = apply_elem<OPT>(wv.y, gv.y, &sv.y, lr, eps);
-        wv.z = apply_elem<OPT>(wv.z, gv.z, &sv.z, lr, eps);
-        wv.w = apply_elem<OPT>(wv.w, gv.w, &sv.w, lr, eps);
-        *reinterpret_cast<float4*>(w + 4 * c) = wv;
-        if (OPT == 1) *reinterpret_cast<float4*>(s + 4 * c) = sv;
+    for (int c0 = lane; c0 < nch; c0 += 8 * kApplyChunks) {
+      float4 gv[kApplyChunks], wv[kApplyChunks], sv[kApplyChunks];
+      bool nz[kApplyChunks];
+#pragma unroll
+      for (int k = 0; k < kApplyChunks; ++k) {
+        const int c = c0 + 8 * k;
+        gv[k] = c < nch ? exch_zero_b128(g + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+#pragma unroll
+      for (int k = 0; k < kApplyChunks; ++k) {
+        const int c = c0 + 8 * k;
+        nz[k] = gv[k].x != 0.f || gv[k].y != 0.f || gv[k].z != 0.f || gv[k].w != 0.f;   // (zero beyond the row)
+        if (nz[k]) {
+          wv[k] = *reinterpret_cast<float4*>(w + 4 * c);
+          sv[k] = (OPT == 1) ? *reinterpret_cast<float4*>(s + 4 * c) : make_float4(0.f, 0.f, 0.f, 0.f);
+        }
+      }
+#pragma unroll
+      for (int k = 0; k < kApplyChunks; ++k) {
+        const int c = c0 + 8 * k;
+        if (nz[k]) {
+          wv[k].x = apply_elem<OPT>(wv[k].x, gv[k].x, &sv[k].x, lr, eps);
+          wv[k].y = apply_elem<OPT>(wv[k].y, gv[k].y, &sv[k].y, lr, eps);
+          wv[k].z = apply_elem<OPT>(wv[k].z, gv[k].z, &sv[k].z, lr, eps);
+          wv[k].w = apply_elem<OPT>(wv[k].w, gv[k].w, &sv[k].w, lr, eps);
+          *reinterpret_cast<float4*>(w + 4 * c) = wv[k];
+          if (OPT == 1) *reinterpret_cast<float4*>(s + 4 * c) = sv[k];
+        }
       }
     }
   } else {
@@ -346,9 +392,9 @@ int launch_apply(const kge_model_t* m, float* const* tables_rw, float* const* gr
     }
   }
   if (T.ntasks == 0) return KGE_OK;
-  const dim3 grid((unsigned)((n + kGroupsPerCta - 1) / kGroupsPerCta), (unsigned)T.ntasks);
-  if (optimizer == 0) apply_rows_kernel<0><<<grid, kThreads, 0, st>>>(T, n, lr, eps);
-  else apply_rows_kernel<1><<<grid, kThreads, 0, st>>>(T, n, lr, eps);
+  const dim3 grid((unsigned)((n + kApplyGroups - 1) / kApplyGroups), (unsigned)T.ntasks);
+  if (optimizer == 0) apply_rows_kernel<0><<<grid, kApplyThreads, 0, st>>>(T, n, lr, eps);
+  else apply_rows_kernel<1><<<grid, kApplyThreads, 0, st>>>(T, n, lr, eps);
   KGE_CHECK_LAUNCH("apply_rows_kernel");
   return KGE_OK;
 }
@@ -450,18 +496,27 @@ extern "C" int kge_train_pairwise_hinge_sgd(const kge_model_t* m, float* const* 
   cudaStream_t st = (cudaStream_t)stream;
   KGE_CUDA_OK(cudaMemsetAsync(loss_out, 0, sizeof(float), st));
   const int sf = (int)group_scratch_floats_bwd(m);
-  const size_t smem = (size_t)sf * kGroupsPerCta * sizeof(float);
-  const unsigned grid = (unsigned)((n + kGroupsPerCta - 1) / kGroupsPerCta);
-#define CALL(M, V)                                                                               \
-  do {                                                                                           \
-    if (smem > 40 * 1024)                                                                        \
-      KGE_CUDA_OK(cudaFuncSetAttribute(train_hinge_kernel<M, V>,                                 \
-                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    train_hinge_kernel<M, V><<<grid, kThreads, smem, st>>>(P, GT, pos_h, pos_r, pos_t, neg_h, neg_r, \
-                                                          neg_t, n, margin, loss_out, sf);       \
+  const size_t smem = (size_t)sf * kHingeGroups * sizeof(float);
+  const unsigned grid = (unsigned)((n + kHingeGroups / 2 - 1) / (kHingeGroups / 2));
+  const int ch = hinge_ch(m->model, vec, ch_select(m->dim));
+#define LAUNCH(M, V, C)                                                                           \
+  do {                                                                                            \
+    if (smem > 40 * 1024)                                                                         \
+      KGE_CUDA_OK(cudaFuncSetAttribute(train_hinge_kernel<M, V, C>,                               \
+                                       cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));  \
+    train_hinge_kernel<M, V, C><<<grid, kHingeThreads, smem, st>>>(P, GT, pos_h, pos_r, pos_t, neg_h, neg_r, \
+                                                                   neg_t, n, margin, loss_out, sf); \
+  } while (0)
+#define CALL(M, V)                                             \
+  do {                                                         \
+    if (ch == 2) { LAUNCH(M, V, hinge_ch(M, V, 2)); }          \
+    else if (ch == 4) { LAUNCH(M, V, hinge_ch(M, V, 4)); }     \
+    else if (ch == 8) { LAUNCH(M, V, hinge_ch(M, V, 8)); }     \
+    else { LAUNCH(M, V, 0); }                                  \
   } while (0)
   KGE_DISPATCH_MODEL_VEC(m->model, vec, CALL);
 #undef CALL
+#undef LAUNCH
   KGE_CHECK_LAUNCH("train_hinge_kernel");
   const int64_t* hs[2] = {pos_h, neg_h};
   const int64_t* rs[2] = {pos_r, neg_r};
