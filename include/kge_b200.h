@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KGE_ABI_VERSION 8
+#define KGE_ABI_VERSION 9
 #define KGE_MAX_TABLES 16
 
 /* status codes */
@@ -336,10 +336,17 @@ int kge_proj_bce(const float* preds, const float* labels, int64_t B, int64_t N, 
  * torch.sparse(...).to_dense() and ships as two [B, N] float tensors.  labels[b, :] = 0 except 1.0 at the
  * entities idx[ptr[row] .. ptr[row+1]) with row = rows[b] (rows == NULL: row = b).  ptr/idx are a CSR of
  * hr_t_train (or tr_h_train) over its distinct keys, rows[b] the key row of training triple b — so a
- * batch moves B ids instead of B*N floats over PCIe.  (The -1 entries the reference adds when
- * neg_rate > 0, used by ProjE only, are not produced.) */
+ * batch moves B ids instead of B*N floats over PCIe.  The -1 entries the reference adds when neg_rate > 0
+ * (ProjE only) come from kge_proj_labels_negatives, called after this. */
 int kge_proj_labels(const int64_t* rows, const int64_t* ptr, const int64_t* idx, int64_t B, int64_t N,
                     float* labels, void* stream);
+
+/* The -1 labels of process_function_multiclass with neg_rate > 0 (pykg2vec/data/generator.py:200-238, used by
+ * ProjE_pointwise): one permutation of the entities per batch, and its first min(100, N) ids are negatives of
+ * every row and both directions unless they are positives of that row.  After kge_proj_labels:
+ *   labels[b, neg[j]] = -1 for b < B, j < n_neg, wherever labels[b, neg[j]] == 0.
+ * neg: n_neg DISTINCT entity ids (device int64).  B = 0 or n_neg = 0 is a no-op. */
+int kge_proj_labels_negatives(float* labels, int64_t B, int64_t N, const int64_t* neg, int64_t n_neg, void* stream);
 
 /* predict_tail_rank / predict_head_rank (projection.py:119-125: topk of -preds over all N entities,
  * one query at a time) + MetricCalculator.get_*_rank (evaluator.py:70-123), for Q queries at once and
@@ -487,6 +494,43 @@ typedef struct kge_acre {
 int64_t kge_acre_trunk_workspace_bytes(const kge_acre_t* p, int64_t Q);
 int kge_acre_trunk_fwd(const kge_acre_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
                        void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- ProjE_pointwise (pykg2vec/models/projection.py:128-257) ------------------------------------
+ * Tables with the reference's state_dict shapes (device fp32): ent [num_ent, k], rel [num_rel, k],
+ * bc1 / De1 / Dr1 / bc2 / De2 / Dr2 [1, k].  k = hidden_size <= 1024 (KGE_ENOTSUP above).
+ *
+ * kge_proje_trunk_fwd: f1 (direction 0, :212-219) or f2 (direction 1, :221-228; plain r, no reciprocal
+ * relation) for Q queries, x[q, :] = tanh(ent[e[q]] * De + rel[r[q]] * Dr + bc), times noise[q, :] when noise
+ * ([Q, k]) is not NULL.  Canonical arithmetic: fmul, fmul, fadd, fadd (no contraction), then the canonical tanh
+ * (DESIGN.md §3).  Evaluation ranks x with kge_proj_rank and bias NULL (g(), :248-257).  Q = 0 is a no-op.
+ *
+ * kge_proje_train_step: forward(e, r, er_e2, direction) of both directions (:194-210) — the dropout noise is
+ * the caller's (torch.dropout(train=True) = x * noise, noise = bernoulli(1 - p) / (1 - p); NULL: no dropout) —
+ * their summed loss Criterion.multi_class (criterion.py:52-55) into loss_out[0], and the backward.  hr_t /
+ * tr_h: the dense [B, num_ent] label rows the Generator yields (1 positive, -1 negative, 0 ignored); either may
+ * be NULL to run one direction only (its ids may then be NULL too).  Only the nonzero labels are evaluated:
+ * the reference's loss gives every zero-label entry exactly zero loss and gradient.  grads[8]: dense
+ * gradient buffers in parameter_list order (ent, rel, bc1, De1, Dr1, bc2, De2, Dr2), ACCUMULATED (caller
+ * zeroes; each may be NULL).  The regulariser is not included: kge_reg_l1_dense.  B = 0 writes a zero loss. */
+typedef struct kge_proje {
+  int32_t hidden_size;
+  int64_t num_ent, num_rel;
+  const float* ent; const float* rel;
+  const float* bc1; const float* De1; const float* Dr1;
+  const float* bc2; const float* De2; const float* Dr2;
+} kge_proje_t;
+int kge_proje_trunk_fwd(const kge_proje_t* p, int32_t direction, const int64_t* e, const int64_t* r, int64_t Q,
+                        const float* noise, float* x, void* stream);
+int kge_proje_train_step(const kge_proje_t* p, const int64_t* h, const int64_t* r, const int64_t* t, int64_t B,
+                         const float* hr_t, const float* tr_h, const float* noise_tail, const float* noise_head,
+                         float* const* grads, float* loss_out, void* stream);
+
+/* ProjE_pointwise.get_reg (projection.py:189-192): an L1 sum over WHOLE tensors, not over batch rows.
+ *   reg_out[0] = lmbda * sum_i sum_j |w[i][j]|   for the `count` (<= 16) tensors w[i] of n[i] floats;
+ *   grad[i][j] += lmbda * sign(w[i][j])          (abs's backward: sign(0) = 0); grad or grad[i] may be NULL.
+ * The sum is an fp32 reduction in no fixed order. */
+int kge_reg_l1_dense(const float* const* w, float* const* grad, const int64_t* n, int32_t count, float lmbda,
+                     float* reg_out, void* stream);
 
 /* ---- negative sampling on the device: replaces the CPU sampler processes ----
  * process_function_pairwise / process_function_pointwise (pykg2vec/data/generator.py:42-158).

@@ -41,6 +41,7 @@ MODEL_MAP = {
     "hyper": ("pykg2vec_b200.projection", "HypER"),
     "interacte": ("pykg2vec_b200.projection", "InteractE"),
     "acre": ("pykg2vec_b200.projection", "AcrE"),
+    "proje_pointwise": ("pykg2vec_b200.projection", "ProjE_pointwise"),
 }
 
 

@@ -11,7 +11,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_build", "libkge_b200.so")
 MAX_TABLES = 16
-ABI_VERSION = 8
+ABI_VERSION = 9
 ENOTSUP = -2   # include/kge_b200.h KGE_ENOTSUP
 
 MODEL_IDS = {
@@ -35,6 +35,7 @@ EXPORTS = [
     "kge_conve_trunk_workspace_bytes", "kge_conve_trunk_fwd", "kge_hyper_trunk_workspace_bytes", "kge_hyper_trunk_fwd",
     "kge_interacte_trunk_workspace_bytes", "kge_interacte_trunk_fwd",
     "kge_acre_trunk_workspace_bytes", "kge_acre_trunk_fwd",
+    "kge_proje_trunk_fwd", "kge_proje_train_step", "kge_reg_l1_dense", "kge_proj_labels_negatives",
     "kge_project_entities", "kge_normalize_rows_to",
 ]
 
@@ -747,6 +748,94 @@ def acre_trunk_fwd(model, e, r, out=None, workspace=None, cap=None):
                                        _ptr(out[q0:q0 + n]), _ptr(workspace), ctypes.c_int64(workspace.numel()),
                                        _stream()), "kge_acre_trunk_fwd")
     return out
+
+
+PROJE_FIELDS = ("ent", "rel", "bc1", "De1", "Dr1", "bc2", "De2", "Dr2")   # = ProjE_pointwise.parameter_list
+
+
+class KgeProje(ctypes.Structure):
+    """kge_proje_t of include/kge_b200.h."""
+    _fields_ = [("hidden_size", ctypes.c_int32), ("num_ent", ctypes.c_int64), ("num_rel", ctypes.c_int64)] + \
+        [(n, ctypes.c_void_p) for n in PROJE_FIELDS]
+
+
+def proje_struct(tables):
+    """a KgeProje over the eight tables in parameter_list order (ent, rel, bc1, De1, Dr1, bc2, De2, Dr2)"""
+    tables = [_dev_f32(t.detach(), n) for t, n in zip(tables, PROJE_FIELDS)]
+    if len(tables) != 8:
+        raise KgeError("ProjE needs its eight tables")
+    p = KgeProje()
+    p.hidden_size, p.num_ent, p.num_rel = int(tables[0].shape[1]), int(tables[0].shape[0]), int(tables[1].shape[0])
+    for n, t in zip(PROJE_FIELDS, tables):
+        setattr(p, n, t.data_ptr())
+    return p
+
+
+def proje_trunk_fwd(tables, e, r, direction=0, noise=None, out=None):
+    """ProjE f1 (direction 0, tail) / f2 (direction 1, head) for ids e, r -> x [Q,k] (times noise [Q,k] if given)"""
+    p = proje_struct(tables)
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    if r.numel() != Q:
+        raise KgeError("e and r must have equal length")
+    if noise is not None and (_dev_f32(noise, "noise").numel() != Q * p.hidden_size):
+        raise KgeError("noise must be [Q, hidden_size]")
+    if out is None:
+        out = torch.empty((Q, p.hidden_size), dtype=torch.float32, device=e.device)
+    check(lib().kge_proje_trunk_fwd(ctypes.byref(p), ctypes.c_int32(direction), _ptr(e), _ptr(r), ctypes.c_int64(Q),
+                                    _ptr(noise), _ptr(out), _stream()), "kge_proje_trunk_fwd")
+    return out
+
+
+def proje_train_step(tables, h, r, t, hr_t, tr_h, grads, noise_tail=None, noise_head=None, loss_out=None):
+    """ProjE forward + loss + backward of both directions (hr_t or tr_h None: that direction is skipped) in one
+    launch.  grads: eight dense buffers shaped like the tables (or None), accumulated.  -> loss [1]"""
+    p = proje_struct(tables)
+    r = _dev_i64(r, "r")
+    B, N, k = r.numel(), p.num_ent, p.hidden_size
+    for ids, lab, nz, name in ((h, hr_t, noise_tail, "tail"), (t, tr_h, noise_head, "head")):
+        if lab is None:
+            continue
+        if _dev_i64(ids, "ids").numel() != B or _dev_f32(lab, "labels").shape != (B, N):
+            raise KgeError("%s direction: ids [B] and labels [B, num_ent] expected" % name)
+        if nz is not None and _dev_f32(nz, "noise").numel() != B * k:
+            raise KgeError("%s direction: noise must be [B, hidden_size]" % name)
+    if loss_out is None:
+        loss_out = torch.empty(1, dtype=torch.float32, device=r.device)
+    for g, w in zip(grads, tables):
+        if g is not None and (_dev_f32(g, "grad").shape != w.shape):
+            raise KgeError("gradient buffers must be shaped like the tables")
+    check(lib().kge_proje_train_step(ctypes.byref(p), _ptr(h if hr_t is not None else None), _ptr(r),
+                                     _ptr(t if tr_h is not None else None), ctypes.c_int64(B), _ptr(hr_t), _ptr(tr_h),
+                                     _ptr(noise_tail if hr_t is not None else None),
+                                     _ptr(noise_head if tr_h is not None else None), _table_ptr_array(grads),
+                                     _ptr(loss_out), _stream()), "kge_proje_train_step")
+    return loss_out
+
+
+def reg_l1_dense(tensors, grads, lmbda, out=None):
+    """lmbda * sum |w| over every element of `tensors` -> [1]; grads (same length, entries may be None; or None)
+    += lmbda * sign(w)"""
+    ts = [_dev_f32(t.detach(), "w") for t in tensors]
+    if len(ts) > MAX_TABLES:
+        raise KgeError("at most %d tensors" % MAX_TABLES)
+    if out is None:
+        out = torch.empty(1, dtype=torch.float32, device=ts[0].device)
+    ws = _table_ptr_array(ts)
+    gs = _table_ptr_array(grads) if grads is not None else None
+    ns = (ctypes.c_int64 * MAX_TABLES)(*[t.numel() for t in ts])
+    check(lib().kge_reg_l1_dense(ws, gs, ns, ctypes.c_int32(len(ts)), ctypes.c_float(lmbda), _ptr(out), _stream()),
+          "kge_reg_l1_dense")
+    return out
+
+
+def proj_labels_negatives(labels, neg):
+    """labels [B,N] (in place): -1 at the distinct entity ids neg wherever the label is still 0"""
+    labels, neg = _dev_f32(labels, "labels"), _dev_i64(neg, "neg")
+    B, N = labels.shape
+    check(lib().kge_proj_labels_negatives(_ptr(labels), ctypes.c_int64(B), ctypes.c_int64(N), _ptr(neg),
+                                          ctypes.c_int64(neg.numel()), _stream()), "kge_proj_labels_negatives")
+    return labels
 
 
 def launch_count():

@@ -1,11 +1,13 @@
 // kge_proj.cu — C-ABI launchers of the projection-model tail (kernels and launch plans:
-// kge_proj.cuh) and of the ConvE, HypER, InteractE and AcrE inference trunks (kge_conve.cuh, kge_hyper.cuh,
+// kge_proj.cuh), of the ConvE, HypER, InteractE and AcrE inference trunks (kge_conve.cuh, kge_hyper.cuh,
 // kge_interacte.cuh, kge_acre.cuh, which reuse the same tiled GEMM — one translation unit so the kernel
-// template is instantiated once).  Declarations and reference citations: include/kge_b200.h.
+// template is instantiated once) and of ProjE_pointwise's trunk, training step and L1 regulariser
+// (kge_proje.cuh).  Declarations and reference citations: include/kge_b200.h.
 #include <cstdlib>
 
 #include "kge_acre.cuh"
 #include "kge_interacte.cuh"
+#include "kge_proje.cuh"
 
 using namespace kge;
 
@@ -445,6 +447,103 @@ int kge_acre_trunk_fwd(const kge_acre_t* p, const int64_t* e, const int64_t* r, 
                                                                       p->bn2_bias, p->bn2_mean, p->bn2_var,
                                                                       p->bn2_eps, x);
   KGE_CHECK_LAUNCH("hyper_fc_combine_kernel");
+  return KGE_OK;
+}
+
+// ---- ProjE_pointwise: trunk, fused training step, L1 regulariser, negative labels ----------
+
+// KGE_OK, or the error code of a malformed / unsupported model struct (message set for `fn`)
+static int proje_check(const kge_proje_t* p, const char* fn) {
+  if (!p || !p->ent || !p->rel || !p->bc1 || !p->De1 || !p->Dr1 || !p->bc2 || !p->De2 || !p->Dr2) {
+    set_error("%s: null pointer", fn);
+    return KGE_EINVAL;
+  }
+  if (p->hidden_size <= 0 || p->num_ent <= 0 || p->num_ent > 0x7fffffffll || p->num_rel <= 0) {
+    set_error("%s: bad shape hidden_size %d num_ent %lld num_rel %lld", fn, p->hidden_size,
+              (long long)p->num_ent, (long long)p->num_rel);
+    return KGE_EINVAL;
+  }
+  if (p->hidden_size > PROJE_MAX_K) {
+    set_error("%s: hidden_size %d exceeds %d", fn, p->hidden_size, PROJE_MAX_K);
+    return KGE_ENOTSUP;
+  }
+  return KGE_OK;
+}
+
+int kge_proje_trunk_fwd(const kge_proje_t* p, int32_t direction, const int64_t* e, const int64_t* r, int64_t Q,
+                        const float* noise, float* x, void* stream) {
+  if (int rc = proje_check(p, "kge_proje_trunk_fwd")) return rc;
+  if (direction != 0 && direction != 1) { set_error("kge_proje_trunk_fwd: direction must be 0 or 1"); return KGE_EINVAL; }
+  if (Q < 0 || Q > (1ll << 30) / p->hidden_size) { set_error("kge_proje_trunk_fwd: bad Q %lld", (long long)Q); return KGE_EINVAL; }
+  if (Q == 0) return KGE_OK;
+  if (!e || !r || !x) { set_error("kge_proje_trunk_fwd: null pointer"); return KGE_EINVAL; }
+  const int k = p->hidden_size;
+  const bool tail = direction == 0;
+  proje_trunk_kernel<<<proj_tiles(Q * k, 256), 256, 0, (cudaStream_t)stream>>>(
+      p->ent, p->rel, tail ? p->De1 : p->De2, tail ? p->Dr1 : p->Dr2, tail ? p->bc1 : p->bc2, e, r, Q, k, noise, x);
+  KGE_CHECK_LAUNCH("proje_trunk_kernel");
+  return KGE_OK;
+}
+
+int kge_proje_train_step(const kge_proje_t* p, const int64_t* h, const int64_t* r, const int64_t* t, int64_t B,
+                         const float* hr_t, const float* tr_h, const float* noise_tail, const float* noise_head,
+                         float* const* grads, float* loss_out, void* stream) {
+  if (int rc = proje_check(p, "kge_proje_train_step")) return rc;
+  if (!loss_out || !grads || (!hr_t && !tr_h)) {
+    set_error("kge_proje_train_step: null loss_out / grads, or neither label matrix");
+    return KGE_EINVAL;
+  }
+  if (B < 0 || B > 0x7fffffffll) { set_error("kge_proje_train_step: bad B %lld", (long long)B); return KGE_EINVAL; }
+  cudaStream_t st = (cudaStream_t)stream;
+  KGE_CUDA_OK(cudaMemsetAsync(loss_out, 0, sizeof(float), st));
+  if (B == 0) return KGE_OK;
+  if (!r || (hr_t && !h) || (tr_h && !t)) { set_error("kge_proje_train_step: null id pointer"); return KGE_EINVAL; }
+  ProjeStep s{};
+  s.ent = p->ent; s.rel = p->rel; s.r = r; s.N = p->num_ent; s.k = p->hidden_size; s.B = (int)B;
+  s.gent = grads[0]; s.grel = grads[1];
+  s.dir[0] = ProjeDir{h, hr_t, noise_tail, p->De1, p->Dr1, p->bc1, grads[3], grads[4], grads[2]};
+  s.dir[1] = ProjeDir{t, tr_h, noise_head, p->De2, p->Dr2, p->bc2, grads[6], grads[7], grads[5]};
+  s.loss = loss_out;
+  int nd = 0;
+  if (hr_t) s.dirs[nd++] = 0;
+  if (tr_h) s.dirs[nd++] = 1;
+  proje_step_kernel<<<dim3((unsigned)B, (unsigned)nd), PROJE_THREADS, 0, st>>>(s);
+  KGE_CHECK_LAUNCH("proje_step_kernel");
+  return KGE_OK;
+}
+
+int kge_reg_l1_dense(const float* const* w, float* const* grad, const int64_t* n, int32_t count, float lmbda,
+                     float* reg_out, void* stream) {
+  if (!w || !n || !reg_out || count < 0 || count > KGE_MAX_TABLES) {
+    set_error("kge_reg_l1_dense: null pointer or bad count %d", (int)count);
+    return KGE_EINVAL;
+  }
+  L1Args a{};
+  long long nmax = 0;
+  for (int i = 0; i < count; ++i) {
+    if (n[i] < 0 || (n[i] > 0 && !w[i])) { set_error("kge_reg_l1_dense: bad tensor %d", i); return KGE_EINVAL; }
+    a.seg[i] = L1Seg{w[i], grad ? grad[i] : nullptr, (long long)n[i]};
+    if (n[i] > nmax) nmax = n[i];
+  }
+  a.lmbda = lmbda; a.out = reg_out;
+  cudaStream_t st = (cudaStream_t)stream;
+  KGE_CUDA_OK(cudaMemsetAsync(reg_out, 0, sizeof(float), st));
+  if (count == 0 || nmax == 0) return KGE_OK;
+  reg_l1_kernel<<<dim3(reg_l1_blocks(nmax, sm_count()), (unsigned)count), 256, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("reg_l1_kernel");
+  return KGE_OK;
+}
+
+int kge_proj_labels_negatives(float* labels, int64_t B, int64_t N, const int64_t* neg, int64_t n_neg, void* stream) {
+  if (B < 0 || N <= 0 || n_neg < 0 || n_neg > N || B > 0x7fffffffll) {
+    set_error("kge_proj_labels_negatives: bad shape B=%lld N=%lld n_neg=%lld", (long long)B, (long long)N,
+              (long long)n_neg);
+    return KGE_EINVAL;
+  }
+  if (B == 0 || n_neg == 0) return KGE_OK;
+  if (!labels || !neg) { set_error("kge_proj_labels_negatives: null pointer"); return KGE_EINVAL; }
+  proj_labels_neg_kernel<<<(unsigned)B, 128, 0, (cudaStream_t)stream>>>(labels, N, neg, (int)n_neg);
+  KGE_CHECK_LAUNCH("proj_labels_neg_kernel");
   return KGE_OK;
 }
 

@@ -10,7 +10,9 @@ of the positives (process_function_pairwise / _pointwise, generator.py:42-158).
 PROJECTION_BASED models (process_function_multiclass, generator.py:160-236) get their two dense
 [batch, tot_entity] label matrices from one kernel per direction (kge_proj_labels) over device CSRs
 of hr_t_train / tr_h_train: the reference assembles them per batch on the host with
-torch.sparse(...).to_dense() and ships 2*B*N floats through the queue and over PCIe.
+torch.sparse(...).to_dense() and ships 2*B*N floats through the queue and over PCIe.  With neg_rate > 0
+(ProjE_pointwise only) one device permutation per batch supplies the shared -1 negatives
+(kge_proj_labels_negatives).
 
 Same interface as the reference class: `Generator(model, config)`, `start_one_epoch(num_batch)`,
 iteration yields the per-batch list (6 id arrays for pairwise, 4 for pointwise, [h, r, t, hr_t,
@@ -54,6 +56,13 @@ def _label_csr(known, first, rel, dev):
     return tuple(torch.from_numpy(a).to(dev) for a in (rows, ptr, idx))
 
 
+def negative_ids(num_ent, generator):
+    """The shared negatives of one ProjE batch (process_function_multiclass with neg_rate > 0, generator.py:200-217):
+    the first min(100, num_ent) ids of one random permutation of the entities, drawn on the generator's device.
+    Every row of both directions gets -1 at these ids unless they are its positives."""
+    return torch.randperm(int(num_ent), device=generator.device, generator=generator)[:min(100, int(num_ent))]
+
+
 class Generator:
     def __init__(self, model, config, seed=0):
         self.model = model
@@ -68,10 +77,13 @@ class Generator:
         self.train = torch.from_numpy(arr).to(dev)
         self._cols = [self.train[:, k].contiguous() for k in range(3)]
         self.slots = None
+        self._negatives = False
         if self.training_strategy == TrainingStrategy.PROJECTION_BASED:
             if int(getattr(config, "neg_rate", 0)) > 0:
-                raise NotImplementedError("device label rows carry positives only (neg_rate must be 0, as in "
-                                          "the ConvE / TuckER / InteractE / HypER / AcrE hyper-parameter files)")
+                if model.model_name.lower() != "proje_pointwise":
+                    raise NotImplementedError("device label rows carry positives only (neg_rate must be 0, as in "
+                                              "the ConvE / TuckER / InteractE / HypER / AcrE hyper-parameter files)")
+                self._negatives = True   # ProjE: -1 labels at the batch's shared random negatives
             kgraph = config.knowledge_graph
             self._hr = _label_csr(kgraph.read_cache_data('hr_t_train'), arr[:, 0], arr[:, 1], dev)
             self._tr = _label_csr(kgraph.read_cache_data('tr_h_train'), arr[:, 2], arr[:, 1], dev)
@@ -110,6 +122,10 @@ class Generator:
             n, N = int(sel.numel()), int(self.config.tot_entity)
             hr_t = _lib.proj_labels(self._hr[0][sel], self._hr[1], self._hr[2], n, N)
             tr_h = _lib.proj_labels(self._tr[0][sel], self._tr[1], self._tr[2], n, N)
+            if self._negatives:
+                neg = negative_ids(N, self._gen)
+                _lib.proj_labels_negatives(hr_t, neg)
+                _lib.proj_labels_negatives(tr_h, neg)
             self.step += 1
             return [ph, pr, pt, hr_t, tr_h]
         layout = 0 if self.training_strategy == TrainingStrategy.PAIRWISE_BASED else 1

@@ -33,6 +33,11 @@ by side and mixed per channel by a Linear gate (parallel way).  Training runs th
 evaluation without autograd runs kge_acre_trunk_fwd — one kernel for gather + bn0 + the three convs (+ residual
 + bn1 + ReLU in the serial way; the gate input in the parallel way, then the gate on the tiled GEMM and bn1 +
 ReLU), then HypER's Linear GEMM and bn2 + ReLU.
+
+ProjE_pointwise (projection.py:128-257) has no bias row and no BatchNorm: its trunk is tanh(e * De + r * Dr + bc),
+and forward() returns the loss itself (-log sigmoid at the positive labels, -log(1 - sigmoid) at the negative
+ones, zero-label entities weighted 0).  forward() is one autograd Function over kge_proje_train_step, which scores
+only the labelled entries of each row; the batched Evaluator ranks kge_proje_trunk_fwd's x with kge_proj_rank.
 """
 import numpy as np
 import torch
@@ -523,4 +528,149 @@ class AcrE(ProjectionModel):
 
     def predict_head_rank(self, e, r, topk=-1):
         _, rank = torch.topk(-self.forward(e, r, direction="head"), k=topk)
+        return rank
+
+
+class ProjEFunction(torch.autograd.Function):
+    """One direction of ProjE_pointwise.forward (projection.py:194-210): the scalar loss term.  Forward and
+    backward both run in kge_proje_train_step during forward(); backward() scales the stored gradients."""
+
+    @staticmethod
+    def forward(ctx, direction, e, r, labels, noise, *tables):
+        _require_cuda(e, r, labels, *tables)
+        tabs = [t.detach() for t in tables]
+        grads = [torch.zeros_like(t) if ctx.needs_input_grad[5 + i] else None for i, t in enumerate(tabs)]
+        tail = direction == "tail"
+        e, r = e.contiguous(), r.contiguous()
+        labels = labels.detach().to(torch.float32).contiguous()
+        noise = noise.contiguous() if noise is not None else None
+        if tail:
+            loss = _lib.proje_train_step(tabs, e, r, None, labels, None, grads, noise_tail=noise)
+        else:
+            loss = _lib.proje_train_step(tabs, None, r, e, None, labels, grads, noise_head=noise)
+        ctx.mask = [g is not None for g in grads]
+        ctx.save_for_backward(*[g for g in grads if g is not None])
+        return loss.squeeze_(0)
+
+    @staticmethod
+    def backward(ctx, gout):
+        saved = iter(ctx.saved_tensors)
+        grads = [next(saved) * gout if m else None for m in ctx.mask]
+        return (None, None, None, None, None, *grads)
+
+
+class L1RegFunction(torch.autograd.Function):
+    """lmbda * sum |w| over whole tensors (ProjE_pointwise.get_reg, projection.py:189-192) via kge_reg_l1_dense."""
+
+    @staticmethod
+    def forward(ctx, lmbda, *tensors):
+        _require_cuda(*tensors)
+        ts = [t.detach() for t in tensors]
+        grads = [torch.zeros_like(t) if ctx.needs_input_grad[1 + i] else None for i, t in enumerate(ts)]
+        out = _lib.reg_l1_dense(ts, grads, float(lmbda))
+        ctx.mask = [g is not None for g in grads]
+        ctx.save_for_backward(*[g for g in grads if g is not None])
+        return out.squeeze_(0)
+
+    @staticmethod
+    def backward(ctx, gout):
+        saved = iter(ctx.saved_tensors)
+        return (None, *[next(saved) * gout if m else None for m in ctx.mask])
+
+
+class ProjE_pointwise(ProjectionModel):
+    """pykg2vec/models/projection.py:128-257 — same kwargs (including the required `device`), the eight
+    NamedEmbedding tables with the reference's names and state_dict keys, xavier_uniform_ in the reference's order
+    (a seeded construction draws the reference's initial weights), parameter_list, loss binding
+    (Criterion.multi_class), f1 / f2 / g and get_reg.
+
+    forward(e, r, er_e2, direction) returns the direction's loss term, as the reference does, through
+    ProjEFunction: the hidden dropout (torch.dropout(train=True) on every call, :201-203) is drawn with torch as
+    ATen draws it, noise = bernoulli(1 - p) / (1 - p), and multiplied in by the kernel.  The head direction is
+    f2(t, r) with plain r (no reciprocal relation).  get_reg is an L1 sum over the whole tables
+    (kge_reg_l1_dense).  proj_query / proj_tail_tables feed the batched Evaluator (eval: no dropout, as
+    predict_*_rank)."""
+
+    def __init__(self, **kwargs):
+        super(ProjE_pointwise, self).__init__(self.__class__.__name__.lower())
+        param_list = ["tot_entity", "tot_relation", "hidden_size", "lmbda", "hidden_dropout"]
+        param_dict = self.load_params(param_list, kwargs)
+        self.__dict__.update(param_dict)
+        k = self.hidden_size
+        self.device = kwargs["device"]
+        self.ent_embeddings = NamedEmbedding("ent_embedding", self.tot_entity, k)
+        self.rel_embeddings = NamedEmbedding("rel_embedding", self.tot_relation, k)
+        self.bc1 = NamedEmbedding("bc1", 1, k)
+        self.De1 = NamedEmbedding("De1", 1, k)
+        self.Dr1 = NamedEmbedding("Dr1", 1, k)
+        self.bc2 = NamedEmbedding("bc2", 1, k)
+        self.De2 = NamedEmbedding("De2", 1, k)
+        self.Dr2 = NamedEmbedding("Dr2", 1, k)
+        self.parameter_list = [self.ent_embeddings, self.rel_embeddings, self.bc1, self.De1, self.Dr1, self.bc2,
+                               self.De2, self.Dr2]
+        for emb in self.parameter_list:   # the reference's order: it fixes the torch draws
+            nn.init.xavier_uniform_(emb.weight)
+        self.loss = Criterion.multi_class
+
+    def kge_proje_tables(self):
+        """the eight weight tensors in parameter_list order (the C-ABI's kge_proje_t / gradient order)"""
+        return [emb.weight for emb in self.parameter_list]
+
+    def kge_reg_tables(self):
+        """(indices into kge_proje_tables(), tensors) of get_reg's L1 sum: De1, Dr1, De2, Dr2, ent, rel"""
+        idx = (3, 4, 6, 7, 0, 1)
+        tabs = self.kge_proje_tables()
+        return idx, [tabs[i] for i in idx]
+
+    def get_reg(self, h, r, t):
+        return L1RegFunction.apply(float(self.lmbda), *self.kge_reg_tables()[1])
+
+    def dropout_noise(self, rows):
+        """[rows, k] noise of torch.dropout(p=hidden_dropout, train=True) drawn as ATen draws it, or None for p = 0"""
+        p = float(self.hidden_dropout)
+        if p == 0.0:
+            return None
+        w = self.ent_embeddings.weight
+        if p >= 1.0:
+            return torch.zeros((rows, self.hidden_size), dtype=torch.float32, device=w.device)
+        return torch.empty((rows, self.hidden_size), dtype=torch.float32, device=w.device).bernoulli_(1 - p).div_(1 - p)
+
+    def forward(self, e, r, er_e2, direction="tail"):
+        assert direction in ("head", "tail"), "Unknown forward direction"
+        _require_cuda(e, r, self.ent_embeddings.weight)
+        return ProjEFunction.apply(direction, e, r, er_e2, self.dropout_noise(e.shape[0]), *self.kge_proje_tables())
+
+    def f1(self, h, r):
+        """tanh(h * De1 + r * Dr1 + bc1) of embedding rows (projection.py:212-219)"""
+        return torch.tanh(h * self.De1.weight + r * self.Dr1.weight + self.bc1.weight)
+
+    def f2(self, t, r):
+        """tanh(t * De2 + r * Dr2 + bc2) of embedding rows (projection.py:221-228)"""
+        return torch.tanh(t * self.De2.weight + r * self.Dr2.weight + self.bc2.weight)
+
+    @staticmethod
+    def g(f, w):
+        """sigmoid(f . w^T) (projection.py:248-257), on kge_proj_tail_fwd"""
+        return ProjTailFunction.apply(f, w, None)
+
+    def proj_query(self, e, r, direction="tail"):
+        """x [b, k] = f1(e, r) (tail) or f2(e, r) (head) by kge_proje_trunk_fwd, for the batched Evaluator and
+        predict_*_rank (no dropout; not differentiable)."""
+        assert direction in ("head", "tail"), "Unknown forward direction"
+        _require_cuda(e, r, self.ent_embeddings.weight)
+        return _lib.proje_trunk_fwd(self.kge_proje_tables(), e.contiguous(), r.contiguous(),
+                                    0 if direction == "tail" else 1)
+
+    def proj_tail_tables(self):
+        """(entity table [N,k], no bias row) of g()"""
+        return self.ent_embeddings.weight, None
+
+    def predict_tail_rank(self, h, r, topk=-1):
+        preds = _lib.proj_tail_fwd(self.proj_query(h, r, "tail"), self.ent_embeddings.weight.detach())
+        _, rank = torch.topk(-preds, k=topk)
+        return rank
+
+    def predict_head_rank(self, t, r, topk=-1):
+        preds = _lib.proj_tail_fwd(self.proj_query(t, r, "head"), self.ent_embeddings.weight.detach())
+        _, rank = torch.topk(-preds, k=topk)
         return rank

@@ -16,6 +16,8 @@ Two execution modes for the same step semantics:
                              dense step bit for bit)
       adam (the CLI default, common.py:50): ... -> kge_optim_apply_dense per table — dense Adam moves
                              every row every step, so its exact form is one HBM-bound sweep per table
+      ProjE_pointwise      : kge_proje_train_step (both directions, labelled entries only) -> kge_reg_l1_dense
+                             -> kge_optim_apply_dense over the eight tables (get_reg touches every element)
   * data-parallel (torch.distributed world > 1, tables replicated; SURVEY.md 8e row 3): config.dp_mode
       "grads": every rank scores ITS batch shard forward + backward into the dense gradient buffers,
                ONE all-reduce per table sums (hinge) / averages (mean-type losses) them over NVLink, then
@@ -54,6 +56,7 @@ class Trainer:
         self._selfadv_fused = True
         self._world = 1
         self._dp = None
+        self._proje = False
 
     def build_model(self):
         """trainer.py:103-144 (optimizer selection; unknown names raise NotImplementedError)."""
@@ -80,6 +83,13 @@ class Trainer:
                 self._state = [torch.zeros_like(t) if t.requires_grad else None for t in tabs]
             if name == "adam":
                 self._state2 = [torch.zeros_like(t) if t.requires_grad else None for t in tabs]
+        self._proje = name in ("sgd", "adagrad", "adam") and getattr(self.config, "fused_step", True) and \
+            self.model.model_name.lower() == "proje_pointwise"
+        if self._proje:
+            tabs = self.model.kge_proje_tables()
+            self._grad_scratch = [torch.zeros_like(t) for t in tabs]
+            self._state = [torch.zeros_like(t) for t in tabs] if name in ("adagrad", "adam") else None
+            self._state2 = [torch.zeros_like(t) for t in tabs] if name == "adam" else None
         self._step = 0
         self._loss_buf = torch.zeros(1, dtype=torch.float32, device=self.config.device)
         import torch.distributed as dist
@@ -253,6 +263,27 @@ class Trainer:
         self._apply(desc, ((h, r, t),), lr)
         return loss
 
+    def _fused_proje(self, ids):
+        """ProjE_pointwise: train_step_projection (trainer.py:159-174) + backward + optimizer.step() as three
+        launch groups: both directions' forward, loss and backward in one kernel, get_reg's L1 sum with its
+        gradient, then one dense optimizer sweep per table."""
+        h, r, t, hr_t, tr_h = ids
+        m = self.model
+        tabs = m.kge_proje_tables()
+        noise_t = m.dropout_noise(h.numel())   # the reference's draw order: tail forward, then head forward
+        noise_h = m.dropout_noise(t.numel())
+        loss = _lib.proje_train_step(tabs, h, r, t, hr_t.to(torch.float32).contiguous(),
+                                     tr_h.to(torch.float32).contiguous(), self._grad_scratch, noise_t, noise_h)
+        idx, reg_tabs = m.kge_reg_tables()
+        reg = _lib.reg_l1_dense(reg_tabs, [self._grad_scratch[i] for i in idx], float(m.lmbda))
+        self._step += 1
+        lr = float(self.config.learning_rate)
+        for k, w in enumerate(tabs):
+            _lib.optim_apply_dense(w, self._grad_scratch[k], self._opt_code(), lr,
+                                   self._state[k] if self._state else None,
+                                   self._state2[k] if self._state2 else None, step=self._step)
+        return loss + reg
+
     # ---- one batch, host ids in, host loss out (trainer.py:269-300) -----------------------------
     def _to_device(self, arrays):
         """Pack the batch's id arrays into one pinned staging buffer and issue ONE H2D copy
@@ -346,6 +377,9 @@ class Trainer:
         strategy = self.model.training_strategy
         if self._dp == "ids":   # replicated update on the all-gathered global batch
             ids = (exchanged or self.exchange_batch_async(ids))()
+        if self._proje:
+            with torch.no_grad():
+                return self._fused_proje(ids)
         if self._fused:
             with torch.no_grad():
                 if strategy == TrainingStrategy.PAIRWISE_BASED:
@@ -396,7 +430,7 @@ class Trainer:
         else:
             ids, nbytes = self._to_device(list(data))
         self.last_h2d_bytes = nbytes
-        if self._fused:
+        if self._fused or self._proje:
             loss = self.train_batch_device(ids)
             if not sync:
                 return loss                # device tensor; float(loss) syncs when the caller wants the value
