@@ -35,7 +35,7 @@
 extern "C" {
 #endif
 
-#define KGE_ABI_VERSION 9
+#define KGE_ABI_VERSION 10
 #define KGE_MAX_TABLES 16
 
 /* status codes */
@@ -531,6 +531,61 @@ int kge_proje_train_step(const kge_proje_t* p, const int64_t* h, const int64_t* 
  * The sum is an fp32 reduction in no fixed order. */
 int kge_reg_l1_dense(const float* const* w, float* const* grad, const int64_t* n, int32_t count, float lmbda,
                      float* reg_out, void* stream);
+
+/* ---- TuckER (pykg2vec/models/projection.py:258-345) ---------------------------------------------
+ * Tables with the reference's state_dict shapes (device fp32): ent [num_ent, d1], rel [num_rel, d2],
+ * W [d2, d1*d1].  d1, d2 <= 256 (KGE_ENOTSUP above; any width below, multiples of 4 or not).  The kernels
+ * replace the trunk of forward() (:310-334): the reference builds one d1 x d1 matrix PER SAMPLE
+ * (rel[r] @ W.view(d2, -1), :321-323) and drops it out; here one core matrix per DISTINCT relation is built and
+ * the dropout mask is applied (explicit mode) or regenerated (counter mode) inside the contraction, so no
+ * [Q, d1, d1] tensor exists.  Summation orders and the mask's counter layout: DESIGN.md §3 (TuckER).
+ *
+ * kge_tucker_cores: M[u, :] = sum_k rel[ids[u], k] * W[k, :] for u < U, out [U, d1*d1] (:321-323 per relation):
+ * one fma chain over k ascending from 0, so M[u] is bit-reproducible and independent of U and of the tiling.
+ *
+ * kge_tucker_trunk_fwd: for q < Q, ehat = normalize(ent[e[q]]) (* noise0[q]) (:318-320); x_pre[j] = sum_i
+ * ehat[i] m1[q][i][j] M[slot[q]][i][j] (:324-326), one fma chain over i ascending; x[q] = normalize(x_pre)
+ * (* noise2[q]) (:327-328).  slot[q] < U is the row of M holding the core matrix of query q's relation (not
+ * checked).  noise0 / noise2: [Q, d1] or NULL.  mask NULL or mode 0: no dropout1.  mode 1: m1 = noise1 [Q, d1, d1]
+ * (bernoulli(1 - p) / (1 - p)).  mode 2: element (q, i, j) is kept iff a Philox-4x32-10 draw keyed on seed at
+ * counter offset + (q*d1 + i)*d1 + j is >= p, kept values are 1 / (1 - p); p = 0 is no mask.  xpre [Q, d1] and
+ * nrm [Q] (both or neither): x_pre and its L2 norm, which the backward reads.
+ *
+ * kge_tucker_trunk_bwd: from gx = d loss / d x [Q, d1] (kge_proj_tail_bwd's grad_x) through noise2 and the
+ * normalisation, grad_ent[e[q]] += the gradient through noise0 and the first normalisation, and
+ * dM[slot[q]][i][j] += ehat[i] m1 g[j].  grad_ent [num_ent, d1] and dM [U, d1*d1] are ACCUMULATED with float
+ * atomics (caller zeroes; each may be NULL).  The mask arguments of the forward regenerate the same mask.
+ *
+ * kge_tucker_cores_bwd: grad_W[k, :] += sum_u rel[ids[u], k] dM[u, :];  grad_rel[ids[u], k] += sum_ij dM[u][ij]
+ * W[k][ij].  Dense buffers shaped like the parameters, accumulated (caller zeroes; each may be NULL).
+ *
+ * kge_tucker_mask1: the mode-2 mask values of (seed, offset, p) as [Q, d1, d1] floats (tests).
+ *
+ * workspace: kge_tucker_workspace_bytes(p, U) bytes for kge_tucker_cores / kge_tucker_cores_bwd (KGE_EWORKSPACE
+ * when short; nothing is written).  Q = 0 / U = 0 are no-ops.  No entry point allocates. */
+typedef struct kge_tucker {
+  int32_t d1, d2;
+  int64_t num_ent, num_rel;
+  const float* ent; const float* rel; const float* W;
+} kge_tucker_t;
+typedef struct kge_tucker_mask {
+  int32_t mode;          /* 0 none, 1 explicit (noise1), 2 counter (seed, offset, p) */
+  const float* noise1;
+  uint64_t seed, offset;
+  float p;
+} kge_tucker_mask_t;
+int64_t kge_tucker_workspace_bytes(const kge_tucker_t* p, int64_t U);
+int kge_tucker_cores(const kge_tucker_t* p, const int64_t* ids, int64_t U, float* M, void* workspace,
+                     int64_t workspace_bytes, void* stream);
+int kge_tucker_trunk_fwd(const kge_tucker_t* p, const float* M, const int64_t* e, const int64_t* slot, int64_t Q,
+                         const float* noise0, const kge_tucker_mask_t* mask, const float* noise2, float* x,
+                         float* xpre, float* nrm, void* stream);
+int kge_tucker_trunk_bwd(const kge_tucker_t* p, const float* M, const int64_t* e, const int64_t* slot, int64_t Q,
+                         const float* noise0, const kge_tucker_mask_t* mask, const float* noise2, const float* gx,
+                         const float* xpre, const float* nrm, float* grad_ent, float* dM, void* stream);
+int kge_tucker_cores_bwd(const kge_tucker_t* p, const int64_t* ids, int64_t U, const float* dM, float* grad_rel,
+                         float* grad_W, void* workspace, int64_t workspace_bytes, void* stream);
+int kge_tucker_mask1(uint64_t seed, uint64_t offset, float p, int64_t Q, int32_t d1, float* out, void* stream);
 
 /* ---- negative sampling on the device: replaces the CPU sampler processes ----
  * process_function_pairwise / process_function_pointwise (pykg2vec/data/generator.py:42-158).

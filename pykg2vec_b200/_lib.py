@@ -11,7 +11,7 @@ import torch
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_build", "libkge_b200.so")
 MAX_TABLES = 16
-ABI_VERSION = 9
+ABI_VERSION = 10
 ENOTSUP = -2   # include/kge_b200.h KGE_ENOTSUP
 
 MODEL_IDS = {
@@ -36,6 +36,8 @@ EXPORTS = [
     "kge_interacte_trunk_workspace_bytes", "kge_interacte_trunk_fwd",
     "kge_acre_trunk_workspace_bytes", "kge_acre_trunk_fwd",
     "kge_proje_trunk_fwd", "kge_proje_train_step", "kge_reg_l1_dense", "kge_proj_labels_negatives",
+    "kge_tucker_workspace_bytes", "kge_tucker_cores", "kge_tucker_trunk_fwd", "kge_tucker_trunk_bwd",
+    "kge_tucker_cores_bwd", "kge_tucker_mask1",
     "kge_project_entities", "kge_normalize_rows_to",
 ]
 
@@ -81,6 +83,7 @@ def lib():
     L.kge_hyper_trunk_workspace_bytes.restype = ctypes.c_int64
     L.kge_interacte_trunk_workspace_bytes.restype = ctypes.c_int64
     L.kge_acre_trunk_workspace_bytes.restype = ctypes.c_int64
+    L.kge_tucker_workspace_bytes.restype = ctypes.c_int64
     if L.kge_abi_version() != ABI_VERSION:
         raise KgeError("libkge_b200.so ABI %d != binding ABI %d" % (L.kge_abi_version(), ABI_VERSION))
     _lib = L
@@ -836,6 +839,143 @@ def proj_labels_negatives(labels, neg):
     check(lib().kge_proj_labels_negatives(_ptr(labels), ctypes.c_int64(B), ctypes.c_int64(N), _ptr(neg),
                                           ctypes.c_int64(neg.numel()), _stream()), "kge_proj_labels_negatives")
     return labels
+
+
+# ---- TuckER (include/kge_b200.h: kge_tucker_*) ---------------------------------------------------
+TUCKER_FIELDS = ("ent", "rel", "W")   # = TuckER.parameter_list
+TUCKER_MASK_NONE, TUCKER_MASK_EXPLICIT, TUCKER_MASK_COUNTER = 0, 1, 2
+
+
+class KgeTucker(ctypes.Structure):
+    """kge_tucker_t of include/kge_b200.h."""
+    _fields_ = [("d1", ctypes.c_int32), ("d2", ctypes.c_int32), ("num_ent", ctypes.c_int64),
+                ("num_rel", ctypes.c_int64)] + [(n, ctypes.c_void_p) for n in TUCKER_FIELDS]
+
+
+class KgeTuckerMask(ctypes.Structure):
+    """kge_tucker_mask_t of include/kge_b200.h."""
+    _fields_ = [("mode", ctypes.c_int32), ("noise1", ctypes.c_void_p), ("seed", ctypes.c_uint64),
+                ("offset", ctypes.c_uint64), ("p", ctypes.c_float)]
+
+
+def tucker_struct(tables):
+    """a KgeTucker over (ent [N,d1], rel [R,d2], W [d2,d1*d1])"""
+    if len(tables) != 3:
+        raise KgeError("TuckER needs its three tables")
+    ent, rel, W = [_dev_f32(t.detach(), n) for t, n in zip(tables, TUCKER_FIELDS)]
+    if ent.dim() != 2 or rel.dim() != 2 or tuple(W.shape) != (rel.shape[1], ent.shape[1] * ent.shape[1]):
+        raise KgeError("TuckER tables must be ent [N,d1], rel [R,d2], W [d2,d1*d1]")
+    p = KgeTucker()
+    p.d1, p.d2, p.num_ent, p.num_rel = int(ent.shape[1]), int(rel.shape[1]), int(ent.shape[0]), int(rel.shape[0])
+    p.ent, p.rel, p.W = ent.data_ptr(), rel.data_ptr(), W.data_ptr()
+    return p
+
+
+def tucker_mask(Q, d1, noise1=None, counter=None):
+    """kge_tucker_mask_t (or None): noise1 [Q,d1,d1] for the explicit mode, counter = (seed, offset, p) for the
+    counter mode."""
+    if noise1 is not None:
+        if counter is not None:
+            raise KgeError("explicit and counter mask are exclusive")
+        if _dev_f32(noise1, "noise1").numel() != Q * d1 * d1:
+            raise KgeError("noise1 must be [Q, d1, d1]")
+        return KgeTuckerMask(TUCKER_MASK_EXPLICIT, noise1.data_ptr(), 0, 0, 0.0)
+    if counter is None:
+        return None
+    seed, offset, p = counter
+    if not 0.0 <= float(p) <= 1.0:
+        raise KgeError("dropout probability must be in [0, 1]")
+    return KgeTuckerMask(TUCKER_MASK_COUNTER, None, int(seed), int(offset), float(p))
+
+
+def _tucker_workspace(p, U, device):
+    n = int(lib().kge_tucker_workspace_bytes(ctypes.byref(p), ctypes.c_int64(U)))
+    return torch.empty(max(n, 16), dtype=torch.uint8, device=device)
+
+
+def tucker_cores(tables, ids, out=None):
+    """M [U, d1*d1]: the core matrix sum_k rel[ids[u], k] W[k] of every relation id in ids (projection.py:321-323,
+    once per relation instead of once per sample)"""
+    p = tucker_struct(tables)
+    ids = _dev_i64(ids, "ids")
+    U = ids.numel()
+    if out is None:
+        out = torch.empty((U, p.d1 * p.d1), dtype=torch.float32, device=ids.device)
+    elif _dev_f32(out, "out").numel() != U * p.d1 * p.d1:
+        raise KgeError("out must be [U, d1*d1]")
+    ws = _tucker_workspace(p, U, ids.device)
+    check(lib().kge_tucker_cores(ctypes.byref(p), _ptr(ids), ctypes.c_int64(U), _ptr(out), _ptr(ws),
+                                 ctypes.c_int64(ws.numel()), _stream()), "kge_tucker_cores")
+    return out
+
+
+def _tucker_trunk_args(p, M, e, slot, noise0, noise2, noise1, counter):
+    M, e, slot = _dev_f32(M, "M"), _dev_i64(e, "e"), _dev_i64(slot, "slot")
+    Q = e.numel()
+    if slot.numel() != Q:
+        raise KgeError("e and slot must have equal length")
+    if M.dim() != 2 or M.shape[1] != p.d1 * p.d1:
+        raise KgeError("M must be [U, d1*d1]")
+    for nz, name in ((noise0, "noise0"), (noise2, "noise2")):
+        if nz is not None and _dev_f32(nz, name).numel() != Q * p.d1:
+            raise KgeError("%s must be [Q, d1]" % name)
+    return M, e, slot, Q, tucker_mask(Q, p.d1, noise1, counter)
+
+
+def tucker_trunk_fwd(tables, M, e, slot, noise0=None, noise2=None, noise1=None, counter=None, save=False):
+    """TuckER's trunk (projection.py:318-328) for entity ids e and core-matrix rows slot -> x [Q,d1], or with
+    save=True (x, xpre [Q,d1], nrm [Q]) for tucker_trunk_bwd.  noise1 / counter: see tucker_mask."""
+    p = tucker_struct(tables)
+    M, e, slot, Q, mask = _tucker_trunk_args(p, M, e, slot, noise0, noise2, noise1, counter)
+    x = torch.empty((Q, p.d1), dtype=torch.float32, device=e.device)
+    xpre = torch.empty_like(x) if save else None
+    nrm = torch.empty(Q, dtype=torch.float32, device=e.device) if save else None
+    check(lib().kge_tucker_trunk_fwd(ctypes.byref(p), _ptr(M), _ptr(e), _ptr(slot), ctypes.c_int64(Q), _ptr(noise0),
+                                     ctypes.byref(mask) if mask is not None else None, _ptr(noise2), _ptr(x),
+                                     _ptr(xpre), _ptr(nrm), _stream()), "kge_tucker_trunk_fwd")
+    return (x, xpre, nrm) if save else x
+
+
+def tucker_trunk_bwd(tables, M, e, slot, gx, xpre, nrm, grad_ent=None, dM=None, noise0=None, noise2=None, noise1=None,
+                     counter=None):
+    """backward of tucker_trunk_fwd: accumulates into grad_ent [N,d1] and dM [U,d1*d1] (each may be None)"""
+    p = tucker_struct(tables)
+    M, e, slot, Q, mask = _tucker_trunk_args(p, M, e, slot, noise0, noise2, noise1, counter)
+    if _dev_f32(gx, "gx").numel() != Q * p.d1 or _dev_f32(xpre, "xpre").numel() != Q * p.d1 or \
+            _dev_f32(nrm, "nrm").numel() != Q:
+        raise KgeError("gx and xpre must be [Q, d1], nrm [Q]")
+    if grad_ent is not None and _dev_f32(grad_ent, "grad_ent").shape != tables[0].shape:
+        raise KgeError("grad_ent must be shaped like the entity table")
+    if dM is not None and _dev_f32(dM, "dM").shape != M.shape:
+        raise KgeError("dM must be shaped like M")
+    check(lib().kge_tucker_trunk_bwd(ctypes.byref(p), _ptr(M), _ptr(e), _ptr(slot), ctypes.c_int64(Q), _ptr(noise0),
+                                     ctypes.byref(mask) if mask is not None else None, _ptr(noise2), _ptr(gx),
+                                     _ptr(xpre), _ptr(nrm), _ptr(grad_ent), _ptr(dM), _stream()),
+          "kge_tucker_trunk_bwd")
+
+
+def tucker_cores_bwd(tables, ids, dM, grad_rel=None, grad_W=None):
+    """backward of tucker_cores: accumulates into grad_rel [R,d2] and grad_W [d2,d1*d1] (each may be None)"""
+    p = tucker_struct(tables)
+    ids = _dev_i64(ids, "ids")
+    U = ids.numel()
+    if _dev_f32(dM, "dM").numel() != U * p.d1 * p.d1:
+        raise KgeError("dM must be [U, d1*d1]")
+    for g, w in ((grad_rel, tables[1]), (grad_W, tables[2])):
+        if g is not None and _dev_f32(g, "grad").shape != w.shape:
+            raise KgeError("gradient buffers must be shaped like the tables")
+    ws = _tucker_workspace(p, U, ids.device)
+    check(lib().kge_tucker_cores_bwd(ctypes.byref(p), _ptr(ids), ctypes.c_int64(U), _ptr(dM), _ptr(grad_rel),
+                                     _ptr(grad_W), _ptr(ws), ctypes.c_int64(ws.numel()), _stream()),
+          "kge_tucker_cores_bwd")
+
+
+def tucker_mask1(seed, offset, p, Q, d1, device="cuda"):
+    """the counter-mode dropout1 mask of (seed, offset, p) as a [Q, d1, d1] float tensor"""
+    out = torch.empty((Q, d1, d1), dtype=torch.float32, device=device)
+    check(lib().kge_tucker_mask1(ctypes.c_uint64(int(seed)), ctypes.c_uint64(int(offset)), ctypes.c_float(p),
+                                 ctypes.c_int64(Q), ctypes.c_int32(d1), _ptr(out), _stream()), "kge_tucker_mask1")
+    return out
 
 
 def launch_count():

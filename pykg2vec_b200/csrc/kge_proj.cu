@@ -1,13 +1,14 @@
 // kge_proj.cu — C-ABI launchers of the projection-model tail (kernels and launch plans:
 // kge_proj.cuh), of the ConvE, HypER, InteractE and AcrE inference trunks (kge_conve.cuh, kge_hyper.cuh,
 // kge_interacte.cuh, kge_acre.cuh, which reuse the same tiled GEMM — one translation unit so the kernel
-// template is instantiated once) and of ProjE_pointwise's trunk, training step and L1 regulariser
-// (kge_proje.cuh).  Declarations and reference citations: include/kge_b200.h.
+// template is instantiated once), of ProjE_pointwise's trunk, training step and L1 regulariser
+// (kge_proje.cuh) and of TuckER's core matrices and trunk, forward and backward (kge_tucker.cuh).  Declarations and reference citations: include/kge_b200.h.
 #include <cstdlib>
 
 #include "kge_acre.cuh"
 #include "kge_interacte.cuh"
 #include "kge_proje.cuh"
+#include "kge_tucker.cuh"
 
 using namespace kge;
 
@@ -544,6 +545,145 @@ int kge_proj_labels_negatives(float* labels, int64_t B, int64_t N, const int64_t
   if (!labels || !neg) { set_error("kge_proj_labels_negatives: null pointer"); return KGE_EINVAL; }
   proj_labels_neg_kernel<<<(unsigned)B, 128, 0, (cudaStream_t)stream>>>(labels, N, neg, (int)n_neg);
   KGE_CHECK_LAUNCH("proj_labels_neg_kernel");
+  return KGE_OK;
+}
+
+// ---- TuckER: core matrices per distinct relation, trunk forward / backward -----------------------
+
+static int tucker_check(const kge_tucker_t* p, const char* fn) {
+  if (!p || !p->ent || !p->rel || !p->W) { set_error("%s: null pointer", fn); return KGE_EINVAL; }
+  if (p->d1 <= 0 || p->d2 <= 0 || p->num_ent <= 0 || p->num_rel <= 0) {
+    set_error("%s: bad shape d1 %d d2 %d num_ent %lld num_rel %lld", fn, p->d1, p->d2, (long long)p->num_ent,
+              (long long)p->num_rel);
+    return KGE_EINVAL;
+  }
+  if (p->d1 > TUCKER_MAX_D || p->d2 > TUCKER_MAX_D) {
+    set_error("%s: d1 %d / d2 %d exceed %d", fn, p->d1, p->d2, TUCKER_MAX_D);
+    return KGE_ENOTSUP;
+  }
+  return KGE_OK;
+}
+
+// U core matrices per call: the GEMM's row-tile grid and 32-bit row count
+static int tucker_check_U(int64_t U, const char* fn) {
+  if (U < 0 || U > 65535ll * PBM) { set_error("%s: bad U %lld", fn, (long long)U); return KGE_EINVAL; }
+  return KGE_OK;
+}
+
+static int tucker_mask(const kge_tucker_mask_t* m, const char* fn, TuckerMask* out) {
+  *out = TuckerMask{};
+  if (!m || m->mode == TUCKER_MASK_NONE) return KGE_OK;
+  if (m->mode == TUCKER_MASK_EXPLICIT) {
+    if (!m->noise1) { set_error("%s: explicit mask without noise1", fn); return KGE_EINVAL; }
+    out->mode = TUCKER_MASK_EXPLICIT; out->noise1 = m->noise1;
+    return KGE_OK;
+  }
+  if (m->mode != TUCKER_MASK_COUNTER || !(m->p >= 0.f)) { set_error("%s: bad mask mode %d / p", fn, m->mode); return KGE_EINVAL; }
+  if (m->p == 0.f) return KGE_OK;   // nothing is dropped: no mask at all
+  out->mode = TUCKER_MASK_COUNTER; out->seed = m->seed; out->offset = m->offset;
+  tucker_mask_params(m->p, &out->thresh, &out->scale);
+  return KGE_OK;
+}
+
+int64_t kge_tucker_workspace_bytes(const kge_tucker_t* p, int64_t U) {
+  if (!p || p->d2 <= 0) return 0;
+  return tucker_workspace_floats(U, p->d2) * (int64_t)sizeof(float);
+}
+
+int kge_tucker_cores(const kge_tucker_t* p, const int64_t* ids, int64_t U, float* M, void* workspace,
+                     int64_t workspace_bytes, void* stream) {
+  if (int rc = tucker_check(p, "kge_tucker_cores")) return rc;
+  if (int rc = tucker_check_U(U, "kge_tucker_cores")) return rc;
+  if (U == 0) return KGE_OK;
+  if (!ids || !M || !workspace) { set_error("kge_tucker_cores: null pointer"); return KGE_EINVAL; }
+  if (workspace_bytes < kge_tucker_workspace_bytes(p, U)) { set_error("kge_tucker_cores: workspace too small"); return KGE_EWORKSPACE; }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* relU = (float*)workspace;
+  tucker_gather_rows_kernel<<<proj_tiles(U * p->d2, 256), 256, 0, st>>>(p->rel, ids, U, p->d2, relU);
+  KGE_CHECK_LAUNCH("tucker_gather_rows_kernel");
+  return launch_gemm<EPI_STORE>(tucker_plan_cores(relU, p->W, U, p->d1, p->d2, M), st, "proj_gemm_kernel<tucker cores>");
+}
+
+static int tucker_trunk_args(const kge_tucker_t* p, const char* fn, const float* M, const int64_t* e,
+                             const int64_t* slot, int64_t Q, const float* noise0, const kge_tucker_mask_t* mask,
+                             const float* noise2, TuckerTrunk* a) {
+  if (int rc = tucker_check(p, fn)) return rc;
+  if (Q < 0 || Q > 0x7fffffffll) { set_error("%s: bad Q %lld", fn, (long long)Q); return KGE_EINVAL; }
+  *a = TuckerTrunk{};
+  if (int rc = tucker_mask(mask, fn, &a->mask)) return rc;
+  if (Q == 0) return KGE_OK;
+  if (!M || !e || !slot) { set_error("%s: null pointer", fn); return KGE_EINVAL; }
+  a->ent = p->ent; a->M = M; a->e = e; a->slot = slot; a->d1 = p->d1; a->noise0 = noise0; a->noise2 = noise2;
+  return KGE_OK;
+}
+
+int kge_tucker_trunk_fwd(const kge_tucker_t* p, const float* M, const int64_t* e, const int64_t* slot, int64_t Q,
+                         const float* noise0, const kge_tucker_mask_t* mask, const float* noise2, float* x,
+                         float* xpre, float* nrm, void* stream) {
+  TuckerTrunk a;
+  if (int rc = tucker_trunk_args(p, "kge_tucker_trunk_fwd", M, e, slot, Q, noise0, mask, noise2, &a)) return rc;
+  if (Q == 0) return KGE_OK;
+  if (!x || (!xpre != !nrm)) { set_error("kge_tucker_trunk_fwd: null x, or only one of xpre / nrm"); return KGE_EINVAL; }
+  a.x = x; a.xpre = xpre; a.nrm = nrm;
+  tucker_trunk_fwd_kernel<<<(unsigned)Q, TUCKER_THREADS, 0, (cudaStream_t)stream>>>(a);
+  KGE_CHECK_LAUNCH("tucker_trunk_fwd_kernel");
+  return KGE_OK;
+}
+
+int kge_tucker_trunk_bwd(const kge_tucker_t* p, const float* M, const int64_t* e, const int64_t* slot, int64_t Q,
+                         const float* noise0, const kge_tucker_mask_t* mask, const float* noise2, const float* gx,
+                         const float* xpre, const float* nrm, float* grad_ent, float* dM, void* stream) {
+  TuckerTrunk a;
+  if (int rc = tucker_trunk_args(p, "kge_tucker_trunk_bwd", M, e, slot, Q, noise0, mask, noise2, &a)) return rc;
+  if (Q == 0 || (!grad_ent && !dM)) return KGE_OK;
+  if (!gx || !xpre || !nrm) { set_error("kge_tucker_trunk_bwd: null pointer"); return KGE_EINVAL; }
+  a.gx = gx; a.xpre = const_cast<float*>(xpre); a.nrm = const_cast<float*>(nrm); a.gent = grad_ent; a.dM = dM;
+  tucker_trunk_bwd_kernel<<<(unsigned)Q, TUCKER_THREADS, 0, (cudaStream_t)stream>>>(a);
+  KGE_CHECK_LAUNCH("tucker_trunk_bwd_kernel");
+  return KGE_OK;
+}
+
+int kge_tucker_cores_bwd(const kge_tucker_t* p, const int64_t* ids, int64_t U, const float* dM, float* grad_rel,
+                         float* grad_W, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (int rc = tucker_check(p, "kge_tucker_cores_bwd")) return rc;
+  if (int rc = tucker_check_U(U, "kge_tucker_cores_bwd")) return rc;
+  if (U == 0 || (!grad_rel && !grad_W)) return KGE_OK;
+  if (!ids || !dM || !workspace) { set_error("kge_tucker_cores_bwd: null pointer"); return KGE_EINVAL; }
+  if (workspace_bytes < kge_tucker_workspace_bytes(p, U)) { set_error("kge_tucker_cores_bwd: workspace too small"); return KGE_EWORKSPACE; }
+  cudaStream_t st = (cudaStream_t)stream;
+  const int d1 = p->d1, d2 = p->d2;
+  float* relU = (float*)workspace;
+  float* drelU = relU + (long long)U * d2;
+  if (grad_W) {
+    tucker_gather_rows_kernel<<<proj_tiles(U * d2, 256), 256, 0, st>>>(p->rel, ids, U, d2, relU);
+    KGE_CHECK_LAUNCH("tucker_gather_rows_kernel");
+    if (int rc = launch_gemm<EPI_ATOMIC>(tucker_plan_grad_W(relU, dM, U, d1, d2, grad_W), st,
+                                         "proj_gemm_kernel<tucker grad_W>")) return rc;
+  }
+  if (grad_rel) {
+    KGE_CUDA_OK(cudaMemsetAsync(drelU, 0, sizeof(float) * (size_t)U * d2, st));
+    if (int rc = launch_gemm<EPI_ATOMIC>(tucker_plan_grad_rel(dM, p->W, U, d1, d2, drelU, 2 * sm_count()), st,
+                                         "proj_gemm_kernel<tucker grad_rel>")) return rc;
+    tucker_scatter_rows_kernel<<<proj_tiles(U * d2, 256), 256, 0, st>>>(drelU, ids, U, d2, grad_rel);
+    KGE_CHECK_LAUNCH("tucker_scatter_rows_kernel");
+  }
+  return KGE_OK;
+}
+
+int kge_tucker_mask1(uint64_t seed, uint64_t offset, float p, int64_t Q, int32_t d1, float* out, void* stream) {
+  if (Q < 0 || d1 <= 0 || d1 > TUCKER_MAX_D || !(p >= 0.f) || Q > (1ll << 40) / ((int64_t)d1 * d1)) {
+    set_error("kge_tucker_mask1: bad shape / p");
+    return KGE_EINVAL;
+  }
+  if (Q == 0) return KGE_OK;
+  if (!out) { set_error("kge_tucker_mask1: null pointer"); return KGE_EINVAL; }
+  TuckerMask m{};
+  m.mode = TUCKER_MASK_COUNTER; m.seed = seed; m.offset = offset;
+  tucker_mask_params(p, &m.thresh, &m.scale);
+  if (p == 0.f) { m.thresh = 0u; m.scale = 1.0f; }
+  const long long n = Q * (long long)d1 * d1;
+  tucker_mask1_kernel<<<proj_tiles(n, 256), 256, 0, (cudaStream_t)stream>>>(m, n, out);
+  KGE_CHECK_LAUNCH("tucker_mask1_kernel");
   return KGE_OK;
 }
 

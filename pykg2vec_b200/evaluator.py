@@ -324,6 +324,11 @@ class Evaluator:
         dev = self._dev()
         Q = hs.shape[0]
         ent, bias = self.model.proj_tail_tables()
+        # TuckER: the core matrices of the relations present, built once for every batch and both directions of
+        # this call (never kept longer: a training step may rewrite the weights behind torch's back)
+        make_cores = getattr(self.model, "proj_query_cores", None)
+        cores = make_cores(torch.from_numpy(np.unique(rs)).to(dev)) if make_cores is not None and Q else None
+        kw = {"cores": cores} if cores is not None else {}
         for lo in range(0, Q, self.QUERY_BATCH):
             hi = min(Q, lo + self.QUERY_BATCH)
             q = hi - lo
@@ -349,8 +354,8 @@ class Evaluator:
             ft = (v[3], v[5]) if filt_t is not None and len(parts[5]) else None
             fh = (v[4], v[6]) if filt_t is not None and len(parts[6]) else None
             counts = torch.zeros((q, 4), dtype=torch.int32, device=dev)
-            x_t = self.model.proj_query(h, r, direction="tail").contiguous()
-            x_h = self.model.proj_query(t, r, direction="head").contiguous()
+            x_t = self.model.proj_query(h, r, direction="tail", **kw).contiguous()
+            x_h = self.model.proj_query(t, r, direction="head", **kw).contiguous()
             bias_row = bias.detach() if bias is not None else None
             _lib.proj_rank(x_t, ent.detach(), bias_row, t, ft, 0, counts)
             _lib.proj_rank(x_h, ent.detach(), bias_row, h, fh, 1, counts)

@@ -34,6 +34,12 @@ evaluation without autograd runs kge_acre_trunk_fwd — one kernel for gather + 
 + bn1 + ReLU in the serial way; the gate input in the parallel way, then the gate on the tiled GEMM and bn1 +
 ReLU), then HypER's Linear GEMM and bn2 + ReLU.
 
+TuckER (projection.py:258-345) has the same tail and loss without a bias row; its trunk contracts the normalised
+entity row with a d1 x d1 core matrix that the relation selects from the core tensor W.  The reference builds that
+matrix per sample; kge_tucker_cores builds it once per distinct relation and kge_tucker_trunk_fwd / _bwd apply the
+dropout on it from a counter, in training (TuckerTrunkFunction, or the Trainer's fused step) and in evaluation
+(proj_query_cores: one set of matrices per Evaluator.rank_triples call).
+
 ProjE_pointwise (projection.py:128-257) has no bias row and no BatchNorm: its trunk is tanh(e * De + r * Dr + bc),
 and forward() returns the loss itself (-log sigmoid at the positive labels, -log(1 - sigmoid) at the negative
 ones, zero-label entities weighted 0).  forward() is one autograd Function over kge_proje_train_step, which scores
@@ -163,13 +169,105 @@ class ConvE(ProjectionModel):
         return rank
 
 
+def _philox_key(device, count):
+    """(seed, offset) of `count` counter-mode draws, taken from torch's CUDA generator of `device`: the seed is the
+    generator's (torch.manual_seed), the offset its Philox offset, which is advanced past the draws as an ATen
+    kernel would, so consecutive calls use disjoint counters and a reseeded run repeats."""
+    gen = torch.cuda.default_generators[device.index if device.index is not None else torch.cuda.current_device()]
+    seed, offset = gen.initial_seed(), gen.get_offset()
+    gen.set_offset(offset + 4 * ((count + 3) // 4))
+    return seed, offset
+
+
+class TuckerTrunkFunction(torch.autograd.Function):
+    """x = TuckER's trunk (projection.py:318-328) on kge_tucker_cores -> kge_tucker_trunk_fwd; backward runs
+    kge_tucker_trunk_bwd -> kge_tucker_cores_bwd.  One core matrix per distinct relation of the batch is built and
+    kept for the backward ([U, d1*d1]); no [B, d1, d1] tensor exists.  mask: None, ("explicit", noise1) or
+    ("counter", seed, offset, p)."""
+
+    @staticmethod
+    def forward(ctx, e, r, noise0, mask, noise2, ent, rel, W):
+        _require_cuda(e, r, ent, rel, W)
+        tabs = [ent.detach().contiguous(), rel.detach().contiguous(), W.detach().contiguous()]
+        ids, slot = torch.unique(r, return_inverse=True)
+        slot = slot.contiguous()
+        kw = {}
+        if mask is not None:
+            kw = {"noise1": mask[1].contiguous()} if mask[0] == "explicit" else {"counter": tuple(mask[1:])}
+        kw.update(noise0=noise0, noise2=noise2)
+        M = _lib.tucker_cores(tabs, ids)
+        x, xpre, nrm = _lib.tucker_trunk_fwd(tabs, M, e.contiguous(), slot, save=True, **kw)
+        ctx.kw = kw
+        ctx.save_for_backward(e.contiguous(), ids, slot, M, xpre, nrm, *tabs)
+        return x
+
+    @staticmethod
+    def backward(ctx, gx):
+        e, ids, slot, M, xpre, nrm, ent, rel, W = ctx.saved_tensors
+        tabs = [ent, rel, W]
+        need = ctx.needs_input_grad[5:8]
+        gent = torch.zeros_like(ent) if need[0] else None
+        dM = torch.zeros_like(M) if (need[1] or need[2]) else None
+        _lib.tucker_trunk_bwd(tabs, M, e, slot, gx.contiguous(), xpre, nrm, gent, dM, **ctx.kw)
+        grel = torch.zeros_like(rel) if need[1] else None
+        gW = torch.zeros_like(W) if need[2] else None
+        if dM is not None:
+            _lib.tucker_cores_bwd(tabs, ids, dM, grel, gW)
+        return None, None, None, None, None, gent, grel, gW
+
+
+class TuckerCores:
+    """The core matrices of a set of relations for evaluation (TuckER.proj_query_cores): built once, reused by every
+    query batch and both directions.  At most `budget_bytes` of matrices are held: when the relations need more,
+    they are split into chunks of budget_bytes // (4 d1^2) relations and the chunk a batch needs is (re)built on
+    demand, one at a time.  A core matrix does not depend on which other relations share its kernel call, so
+    chunking never changes x.  The matrices are a snapshot of rel and W: do not keep this object across a weight
+    update (the fused optimizer kernels write through raw pointers, which torch's version counters do not see)."""
+
+    def __init__(self, tables, rel_ids, budget_bytes):
+        self.tables = [t.detach() for t in tables]
+        d1 = self.tables[0].shape[1]
+        self.ids = torch.unique(rel_ids)   # sorted
+        self.per = max(1, int(budget_bytes) // (4 * d1 * d1))
+        self.builds = 0
+        self._chunk = (-1, None)
+        if self.ids.numel() <= self.per:
+            self._cores(0)
+
+    def _cores(self, c):
+        if self._chunk[0] != c:
+            self._chunk = (-1, None)   # release the held chunk before the next one is allocated
+            self._chunk = (c, _lib.tucker_cores(self.tables, self.ids[c * self.per:(c + 1) * self.per].contiguous()))
+            self.builds += 1
+        return self._chunk[1]
+
+    def query(self, e, r):
+        """x [Q, d1] for entity ids e and relation ids r (every r must be among the ids given at construction)"""
+        slot = torch.searchsorted(self.ids, r)
+        if self.ids.numel() <= self.per:
+            return _lib.tucker_trunk_fwd(self.tables, self._cores(0), e, slot)
+        x = torch.empty((e.numel(), self.tables[0].shape[1]), dtype=torch.float32, device=e.device)
+        chunk = torch.div(slot, self.per, rounding_mode="floor")
+        for c in torch.unique(chunk).tolist():
+            idx = (chunk == c).nonzero().flatten()
+            x[idx] = _lib.tucker_trunk_fwd(self.tables, self._cores(c), e[idx].contiguous(),
+                                           (slot[idx] - c * self.per).contiguous())
+        return x
+
+
 class TuckER(ProjectionModel):
     """pykg2vec/models/projection.py:258-345 — same kwargs, tables (ent_embeddings, rel_embeddings, W),
-    parameter_list and loss binding.  The trunk (normalise, contract the relation with the core tensor,
-    multiply, normalise) is a handful of small dense ops and stays on torch; the product against every
-    entity, its loss and the evaluation ranks are the kge_proj_* kernels (no bias row).  As in the
-    reference the `direction` argument is validated and otherwise ignored: both directions apply the
-    same function, to (h, r) and to (t, r)."""
+    parameter_list and loss binding.  As in the reference the `direction` argument is validated and otherwise
+    ignored: both directions apply the same function, to (h, r) and to (t, r).
+
+    The trunk (normalise, contract the relation with the core tensor, multiply, normalise) runs on the kge_tucker_*
+    kernels: one core matrix per distinct relation instead of the reference's one per sample, the dropout on it
+    regenerated from a counter.  With autograd (or in training mode) it is TuckerTrunkFunction; in evaluation
+    without autograd proj_query takes the matrices from a TuckerCores (proj_query_cores).  The reference's torch
+    layers stay as _trunk_layers: the yardstick of the tests, the path for widths the kernels refuse (d1 or
+    d2 > 256) and, with the attribute / kwarg kge_trunk = False, for everything."""
+
+    CORES_BUDGET = 256 << 20   # bytes of core matrices a TuckerCores holds at a time
 
     def __init__(self, **kwargs):
         super(TuckER, self).__init__(self.__class__.__name__.lower())
@@ -189,16 +287,72 @@ class TuckER(ProjectionModel):
         self.hidden_dropout1 = nn.Dropout(self.hidden_dropout1)
         self.hidden_dropout2 = nn.Dropout(self.hidden_dropout2)
         self.loss = Criterion.multi_class_bce
+        self.kge_trunk = bool(kwargs.get("kge_trunk", True))
 
-    def proj_query(self, e1, r, direction="tail"):
-        assert direction in ("head", "tail"), "Unknown forward direction"
-        _require_cuda(e1, r, self.ent_embeddings.weight)
+    def _kernel_trunk(self):
+        """the kernels are selected and the tables live on a CUDA device (the kernels read device memory only)"""
+        return self.kge_trunk and self.ent_embeddings.weight.is_cuda
+
+    def kge_tucker_tables(self):
+        """the three weight tensors in parameter_list order (the C-ABI's kge_tucker_t order)"""
+        return [emb.weight for emb in self.parameter_list]
+
+    # ---- trunk: TuckER.forward before the x . E^T product (projection.py:318-328) ----
+    def _trunk_layers(self, e1, r):
         e1 = torch.nn.functional.normalize(self.ent_embeddings(e1), p=2, dim=1)
         e1 = self.inp_drop(e1).view(-1, 1, self.d1)
         W_mat = torch.matmul(self.rel_embeddings(r), self.W.weight.view(self.d2, -1)).view(-1, self.d1, self.d1)
         W_mat = self.hidden_dropout1(W_mat)
         x = torch.matmul(e1, W_mat).view(-1, self.d1)
         return self.hidden_dropout2(torch.nn.functional.normalize(x, p=2, dim=1))
+
+    def dropout_noise(self, rows, p):
+        """[rows, d1] noise of nn.Dropout(p) in training mode drawn as ATen draws it, or None when nothing drops"""
+        p = float(p)
+        if p == 0.0 or not self.training:
+            return None
+        w = self.ent_embeddings.weight
+        if p >= 1.0:
+            return torch.zeros((rows, self.d1), dtype=torch.float32, device=w.device)
+        return torch.empty((rows, self.d1), dtype=torch.float32, device=w.device).bernoulli_(1 - p).div_(1 - p)
+
+    def dropout1_key(self, rows):
+        """the counter-mode mask ("counter", seed, offset, p) of hidden_dropout1 over [rows, d1, d1], or None"""
+        p = float(self.hidden_dropout1.p)
+        if p == 0.0 or not self.training:
+            return None
+        return ("counter",) + _philox_key(self.ent_embeddings.weight.device, rows * self.d1 * self.d1) + (p,)
+
+    def proj_query_cores(self, rel_ids, budget_bytes=None):
+        """The core matrices of the distinct relations in rel_ids (device int64) for proj_query(..., cores=...), or
+        None when proj_query would not use them (autograd or training mode, kge_trunk off, unsupported widths).
+        Build one per evaluation call, never keep it across a weight update."""
+        if self.training or torch.is_grad_enabled() or not self._kernel_trunk():
+            return None
+        try:
+            return TuckerCores(self.kge_tucker_tables(), rel_ids,
+                               self.CORES_BUDGET if budget_bytes is None else budget_bytes)
+        except _lib.KgeNotSupported:
+            return None
+
+    def proj_query(self, e1, r, direction="tail", cores=None):
+        assert direction in ("head", "tail"), "Unknown forward direction"
+        _require_cuda(e1, r, self.ent_embeddings.weight)
+        if not self._kernel_trunk():
+            return self._trunk_layers(e1, r)
+        e1, r = e1.contiguous(), r.contiguous()
+        try:
+            if not self.training and not torch.is_grad_enabled():
+                cores = cores if cores is not None else self.proj_query_cores(r)
+                if cores is None:
+                    return self._trunk_layers(e1, r)
+                return cores.query(e1, r)
+            rows = e1.shape[0]
+            return TuckerTrunkFunction.apply(e1, r, self.dropout_noise(rows, self.inp_drop.p), self.dropout1_key(rows),
+                                             self.dropout_noise(rows, self.hidden_dropout2.p),
+                                             *self.kge_tucker_tables())
+        except _lib.KgeNotSupported:   # d1 or d2 beyond the kernels' bound
+            return self._trunk_layers(e1, r)
 
     def proj_tail_tables(self):
         return self.ent_embeddings.weight, None

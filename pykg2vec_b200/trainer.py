@@ -18,6 +18,8 @@ Two execution modes for the same step semantics:
                              every row every step, so its exact form is one HBM-bound sweep per table
       ProjE_pointwise      : kge_proje_train_step (both directions, labelled entries only) -> kge_reg_l1_dense
                              -> kge_optim_apply_dense over the eight tables (get_reg touches every element)
+      TuckER               : kge_tucker_cores (one core matrix per distinct relation) -> kge_tucker_trunk_fwd ->
+                             tail + BCE -> kge_tucker_trunk_bwd -> kge_tucker_cores_bwd -> kge_optim_apply_dense
   * data-parallel (torch.distributed world > 1, tables replicated; SURVEY.md 8e row 3): config.dp_mode
       "grads": every rank scores ITS batch shard forward + backward into the dense gradient buffers,
                ONE all-reduce per table sums (hinge) / averages (mean-type losses) them over NVLink, then
@@ -57,6 +59,7 @@ class Trainer:
         self._world = 1
         self._dp = None
         self._proje = False
+        self._tucker = False
 
     def build_model(self):
         """trainer.py:103-144 (optimizer selection; unknown names raise NotImplementedError)."""
@@ -87,6 +90,14 @@ class Trainer:
             self.model.model_name.lower() == "proje_pointwise"
         if self._proje:
             tabs = self.model.kge_proje_tables()
+            self._grad_scratch = [torch.zeros_like(t) for t in tabs]
+            self._state = [torch.zeros_like(t) for t in tabs] if name in ("adagrad", "adam") else None
+            self._state2 = [torch.zeros_like(t) for t in tabs] if name == "adam" else None
+        self._tucker = name in ("sgd", "adagrad", "adam") and getattr(self.config, "fused_step", True) and \
+            self.model.model_name.lower() == "tucker" and self.model._kernel_trunk() and \
+            max(self.model.d1, self.model.d2) <= 256   # beyond the kernels' widths: the autograd path on torch layers
+        if self._tucker:
+            tabs = self.model.kge_tucker_tables()
             self._grad_scratch = [torch.zeros_like(t) for t in tabs]
             self._state = [torch.zeros_like(t) for t in tabs] if name in ("adagrad", "adam") else None
             self._state2 = [torch.zeros_like(t) for t in tabs] if name == "adam" else None
@@ -284,6 +295,48 @@ class Trainer:
                                    self._state2[k] if self._state2 else None, step=self._step)
         return loss + reg
 
+    def _fused_tucker(self, ids):
+        """TuckER: train_step_projection (trainer.py:159-174) + backward + optimizer.step() without an autograd graph.
+        The core matrices of the batch's distinct relations are built once and serve both directions (the relation
+        ids are the same), which run as ONE trunk launch over 2B queries; then the shared tail, the BCE loss and its
+        gradient per direction, the tail's backward, the trunk's, the cores', and one dense optimizer sweep per
+        table.  torch.unique sizes its result on the host: one synchronisation per step."""
+        h, r, t, hr_t, tr_h = ids
+        m = self.model
+        tabs = [w.detach() for w in m.kge_tucker_tables()]
+        ent = tabs[0]
+        B, N = r.numel(), ent.shape[0]
+        uids, slot = torch.unique(r, return_inverse=True)
+        M = _lib.tucker_cores(tabs, uids)
+        e2, slot2 = torch.cat([h, t]), torch.cat([slot, slot])   # rows [0, B): tail direction, [B, 2B): head
+        kw = dict(noise0=m.dropout_noise(2 * B, m.inp_drop.p), noise2=m.dropout_noise(2 * B, m.hidden_dropout2.p))
+        key = m.dropout1_key(2 * B)
+        if key is not None:
+            kw["counter"] = key[1:]
+        x, xpre, nrm = _lib.tucker_trunk_fwd(tabs, M, e2, slot2, save=True, **kw)
+        preds = _lib.proj_tail_fwd(x, ent)
+        scale, shift = 1.0, 0.0
+        if hasattr(self.config, "label_smoothing"):
+            scale, shift = 1.0 - self.config.label_smoothing, 1.0 / self.config.tot_entity
+        gent, grel, gW = self._grad_scratch
+        gx = torch.zeros_like(x)
+        loss = None
+        for lo, lab in ((0, hr_t), (B, tr_h)):
+            part, gp = _lib.proj_bce(preds[lo:lo + B], lab.to(torch.float32).contiguous(), scale, shift)
+            _lib.proj_tail_bwd(gp, preds[lo:lo + B], x[lo:lo + B], ent, gx[lo:lo + B], gent)
+            loss = part if loss is None else loss + part
+        del preds, gp   # the [B, N] buffers go back to the allocator before the U matrices of dM are taken
+        dM = torch.zeros_like(M)
+        _lib.tucker_trunk_bwd(tabs, M, e2, slot2, gx, xpre, nrm, gent, dM, **kw)
+        _lib.tucker_cores_bwd(tabs, uids, dM, grel, gW)
+        self._step += 1
+        lr = float(self.config.learning_rate)
+        for k, w in enumerate(tabs):
+            _lib.optim_apply_dense(w, self._grad_scratch[k], self._opt_code(), lr,
+                                   self._state[k] if self._state else None,
+                                   self._state2[k] if self._state2 else None, step=self._step)
+        return loss
+
     # ---- one batch, host ids in, host loss out (trainer.py:269-300) -----------------------------
     def _to_device(self, arrays):
         """Pack the batch's id arrays into one pinned staging buffer and issue ONE H2D copy
@@ -380,6 +433,9 @@ class Trainer:
         if self._proje:
             with torch.no_grad():
                 return self._fused_proje(ids)
+        if self._tucker:
+            with torch.no_grad():
+                return self._fused_tucker(ids)
         if self._fused:
             with torch.no_grad():
                 if strategy == TrainingStrategy.PAIRWISE_BASED:
@@ -430,7 +486,7 @@ class Trainer:
         else:
             ids, nbytes = self._to_device(list(data))
         self.last_h2d_bytes = nbytes
-        if self._fused or self._proje:
+        if self._fused or self._proje or self._tucker:
             loss = self.train_batch_device(ids)
             if not sync:
                 return loss                # device tensor; float(loss) syncs when the caller wants the value
