@@ -372,7 +372,7 @@ int kge_proj_rank(const float* x, const float* ent, const float* bias, int64_t Q
  *   bn0_* [1], conv_weight [32,1,3,3], conv_bias [32], bn1_* [32], fc_weight [k, F], fc_bias [k],
  *   F = 32 * (2*hidden_size_2 - 2) * (hidden_size_1 - 2), hidden_size_2 = hidden_size / hidden_size_1.
  * x is [Q,k]; workspace >= kge_conve_trunk_workspace_bytes() bytes (the flattened feature maps).
- * Training (batch statistics, dropout, autograd) stays with the framework's own layers. */
+ * Training (batch statistics, dropout, autograd): kge_conve_train_* below. */
 typedef struct kge_conve {
   int32_t hidden_size, hidden_size_1;
   float bn0_eps, bn1_eps;
@@ -385,6 +385,47 @@ typedef struct kge_conve {
 int64_t kge_conve_trunk_workspace_bytes(const kge_conve_t* p, int64_t Q);
 int kge_conve_trunk_fwd(const kge_conve_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
                         void* workspace, int64_t workspace_bytes, void* stream);
+
+/* ---- ConvE trunk, training mode ------------------------------------------------------------
+ * ConvE.inner_forward up to the x.E^T product (pykg2vec/models/projection.py:86-99) with self.training == True,
+ * forward and backward; replaces the reference's torch layers bn0 -> inp_drop -> conv2d_1 -> bn1 -> relu ->
+ * feat_drop -> fc -> hidden_drop -> bn2 -> relu and their autograd.  The Q = G * B rows are G groups of B rows
+ * (G = 2: the tail and head forwards of train_step_projection, trainer.py:159-174, as one call); every BatchNorm
+ * uses the batch statistics of its own group, and the running statistics are updated group after group exactly
+ * as G sequential nn.BatchNorm calls do (momentum from the struct, unbiased variance n / (n - 1));
+ * num_batches_tracked is the caller's.  Running-statistic pointers: all six set, or all NULL (no update).
+ * Dropout is explicit noise, bernoulli(1 - p) / (1 - p) as torch draws it (each may be NULL = no dropout):
+ *   noise0 [Q, 2k] (inp_drop), noise1 [Q, 32] (feat_drop, Dropout2d: one value per channel), noise2 [Q, k].
+ * Images: as kge_conve_trunk_fwd (2k <= 4096, hidden_size_1 >= 3, hidden_size_2 >= 2; KGE_ENOTSUP beyond);
+ * B >= 2 (a one-row BatchNorm1d raises in the reference) and Q a multiple of B, else KGE_EINVAL.
+ *
+ * kge_conve_train_fwd: x [Q, k].  Every statistic is reduced in a fixed order that does not depend on the grid
+ * (DESIGN.md §3, ConvE training), so x and the running statistics are bit-reproducible.  The workspace
+ * (kge_conve_train_workspace_bytes(p, Q, B) bytes) keeps what the backward reads: pass the same workspace, unmodified,
+ * to kge_conve_train_bwd.
+ * kge_conve_train_bwd: from gx = d loss / d x [Q, k] (kge_proj_tail_bwd's grad_x) and the forward's x, ACCUMULATES
+ * into KGE_CONVE_TRAIN_GRADS dense buffers shaped like the parameters (caller zeroes; none may be NULL), in
+ * ConvE.parameters() order without the tail's bias row: ent, rel, bn0.weight, bn0.bias, conv2d_1.weight,
+ * conv2d_1.bias, bn1.weight, bn1.bias, fc.weight, fc.bias, bn2.weight, bn2.bias.  The entity / relation rows are
+ * scattered with float atomics (ids repeat); every other sum runs in a fixed order.  No entry point allocates. */
+#define KGE_CONVE_TRAIN_GRADS 12
+typedef struct kge_conve_train {
+  int32_t hidden_size, hidden_size_1;
+  float bn0_eps, bn1_eps, bn2_eps;
+  float bn0_momentum, bn1_momentum, bn2_momentum;
+  const float* ent; const float* rel;
+  const float* bn0_weight; const float* bn0_bias; const float* conv_weight; const float* conv_bias;
+  const float* bn1_weight; const float* bn1_bias; const float* fc_weight; const float* fc_bias;
+  const float* bn2_weight; const float* bn2_bias;
+  float* bn0_mean; float* bn0_var; float* bn1_mean; float* bn1_var; float* bn2_mean; float* bn2_var;
+} kge_conve_train_t;
+int64_t kge_conve_train_workspace_bytes(const kge_conve_train_t* p, int64_t Q, int64_t B);
+int kge_conve_train_fwd(const kge_conve_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                        const float* noise0, const float* noise1, const float* noise2, float* x, void* workspace,
+                        int64_t workspace_bytes, void* stream);
+int kge_conve_train_bwd(const kge_conve_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                        const float* noise0, const float* noise1, const float* noise2, const float* gx,
+                        const float* x, float* const* grads, void* workspace, int64_t workspace_bytes, void* stream);
 
 /* ---- HypER trunk, inference mode -----------------------------------------------------------
  * HypER.forward up to the x.E^T product (pykg2vec/models/projection.py:581-606) with

@@ -38,6 +38,7 @@ EXPORTS = [
     "kge_proje_trunk_fwd", "kge_proje_train_step", "kge_reg_l1_dense", "kge_proj_labels_negatives",
     "kge_tucker_workspace_bytes", "kge_tucker_cores", "kge_tucker_trunk_fwd", "kge_tucker_trunk_bwd",
     "kge_tucker_cores_bwd", "kge_tucker_mask1",
+    "kge_conve_train_workspace_bytes", "kge_conve_train_fwd", "kge_conve_train_bwd",
     "kge_project_entities", "kge_normalize_rows_to",
 ]
 
@@ -84,8 +85,13 @@ def lib():
     L.kge_interacte_trunk_workspace_bytes.restype = ctypes.c_int64
     L.kge_acre_trunk_workspace_bytes.restype = ctypes.c_int64
     L.kge_tucker_workspace_bytes.restype = ctypes.c_int64
+    L.kge_conve_train_workspace_bytes.restype = ctypes.c_int64
     if L.kge_abi_version() != ABI_VERSION:
         raise KgeError("libkge_b200.so ABI %d != binding ABI %d" % (L.kge_abi_version(), ABI_VERSION))
+    missing = [name for name in EXPORTS if not hasattr(L, name)]
+    if missing:   # a library built before entry points were added to this ABI version: rebuild it
+        raise KgeError("libkge_b200.so at %s lacks %s — rebuild it (python -m pykg2vec_b200.build)"
+                       % (LIB_PATH, ", ".join(missing)))
     _lib = L
     return L
 
@@ -976,6 +982,91 @@ def tucker_mask1(seed, offset, p, Q, d1, device="cuda"):
     check(lib().kge_tucker_mask1(ctypes.c_uint64(int(seed)), ctypes.c_uint64(int(offset)), ctypes.c_float(p),
                                  ctypes.c_int64(Q), ctypes.c_int32(d1), _ptr(out), _stream()), "kge_tucker_mask1")
     return out
+
+
+# ---- ConvE training-mode trunk (include/kge_b200.h: kge_conve_train_*) ------------------------------------------
+CONVE_TRAIN_PARAMS = ("ent", "rel", "bn0_weight", "bn0_bias", "conv_weight", "conv_bias", "bn1_weight", "bn1_bias",
+                      "fc_weight", "fc_bias", "bn2_weight", "bn2_bias")   # = the gradient order of kge_conve_train_bwd
+CONVE_TRAIN_RUNNING = ("bn0_mean", "bn0_var", "bn1_mean", "bn1_var", "bn2_mean", "bn2_var")
+
+
+class KgeConveTrain(ctypes.Structure):
+    """kge_conve_train_t of include/kge_b200.h."""
+    _fields_ = [("hidden_size", ctypes.c_int32), ("hidden_size_1", ctypes.c_int32)] + \
+               [(n, ctypes.c_float) for n in ("bn0_eps", "bn1_eps", "bn2_eps", "bn0_momentum", "bn1_momentum",
+                                              "bn2_momentum")] + \
+               [(n, ctypes.c_void_p) for n in CONVE_TRAIN_PARAMS + CONVE_TRAIN_RUNNING]
+
+
+def conve_train_struct(model, params=None, running=True):
+    """kge_conve_train_t of a ConvE (the reference's sub-module names).  params: the 12 tensors of CONVE_TRAIN_PARAMS
+    (default: the model's own); running=False leaves the running statistics alone (NULL pointers)."""
+    if params is None:
+        params = model.kge_conve_params()
+    if len(params) != len(CONVE_TRAIN_PARAMS):
+        raise KgeError("ConvE's training trunk needs its %d parameter tensors" % len(CONVE_TRAIN_PARAMS))
+    p = KgeConveTrain()
+    p.hidden_size, p.hidden_size_1 = int(model.hidden_size), int(model.hidden_size_1)
+    bns = (model.bn0, model.bn1, model.bn2)
+    p.bn0_eps, p.bn1_eps, p.bn2_eps = (float(bn.eps) for bn in bns)
+    if any(bn.momentum is None for bn in bns):   # cumulative averaging: the torch layers' job
+        raise KgeNotSupported("kge_conve_train: BatchNorm momentum None is not supported")
+    p.bn0_momentum, p.bn1_momentum, p.bn2_momentum = (float(bn.momentum) for bn in bns)
+    for name, t in zip(CONVE_TRAIN_PARAMS, params):
+        setattr(p, name, _dev_f32(t.detach(), name).data_ptr())
+    if running:
+        for i, bn in enumerate(bns):
+            setattr(p, "bn%d_mean" % i, _dev_f32(bn.running_mean, "running_mean").data_ptr())
+            setattr(p, "bn%d_var" % i, _dev_f32(bn.running_var, "running_var").data_ptr())
+    return p
+
+
+def _conve_train_noise(noise, rows, width, name):
+    if noise is not None and (_dev_f32(noise, name).numel() != rows * width):
+        raise KgeError("%s must be [Q, %d]" % (name, width))
+    return _ptr(noise)
+
+
+def conve_train_fwd(model, e, r, B, noise0=None, noise1=None, noise2=None, params=None, running=True):
+    """ConvE's trunk in training mode (projection.py:86-99) on Q = G * B rows, G groups of B with their own batch
+    statistics -> (x [Q, k], workspace).  Updates the model's running statistics in place (group after group) unless
+    running=False; num_batches_tracked is the caller's.  Keep the workspace for conve_train_bwd."""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    if r.numel() != Q:
+        raise KgeError("e and r must have equal length")
+    p = conve_train_struct(model, params, running)
+    k = p.hidden_size
+    n0 = _conve_train_noise(noise0, Q, 2 * k, "noise0")
+    n1 = _conve_train_noise(noise1, Q, 32, "noise1")
+    n2 = _conve_train_noise(noise2, Q, k, "noise2")
+    nbytes = int(lib().kge_conve_train_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q), ctypes.c_int64(B)))
+    ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=e.device)
+    x = torch.empty((Q, k), dtype=torch.float32, device=e.device)
+    check(lib().kge_conve_train_fwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0, n1,
+                                    n2, _ptr(x), _ptr(ws), ctypes.c_int64(ws.numel()), _stream()),
+          "kge_conve_train_fwd")
+    return x, ws
+
+
+def conve_train_bwd(model, e, r, B, gx, x, grads, workspace, noise0=None, noise1=None, noise2=None, params=None):
+    """backward of conve_train_fwd: accumulates into grads, 12 buffers shaped like CONVE_TRAIN_PARAMS"""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    p = conve_train_struct(model, params, running=False)
+    params = params if params is not None else model.kge_conve_params()
+    k = p.hidden_size
+    if _dev_f32(gx, "gx").numel() != Q * k or _dev_f32(x, "x").numel() != Q * k:
+        raise KgeError("gx and x must be [Q, k]")
+    if len(grads) != len(CONVE_TRAIN_PARAMS) or any(_dev_f32(g, "grad").shape != w.shape for g, w in zip(grads, params)):
+        raise KgeError("grads must be %d buffers shaped like the parameters" % len(CONVE_TRAIN_PARAMS))
+    n0 = _conve_train_noise(noise0, Q, 2 * k, "noise0")
+    n1 = _conve_train_noise(noise1, Q, 32, "noise1")
+    n2 = _conve_train_noise(noise2, Q, k, "noise2")
+    arr = (ctypes.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
+    check(lib().kge_conve_train_bwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0, n1,
+                                    n2, _ptr(gx), _ptr(x), arr, _ptr(workspace), ctypes.c_int64(workspace.numel()),
+                                    _stream()), "kge_conve_train_bwd")
 
 
 def launch_count():

@@ -2,10 +2,13 @@
 // kge_proj.cuh), of the ConvE, HypER, InteractE and AcrE inference trunks (kge_conve.cuh, kge_hyper.cuh,
 // kge_interacte.cuh, kge_acre.cuh, which reuse the same tiled GEMM — one translation unit so the kernel
 // template is instantiated once), of ProjE_pointwise's trunk, training step and L1 regulariser
-// (kge_proje.cuh) and of TuckER's core matrices and trunk, forward and backward (kge_tucker.cuh).  Declarations and reference citations: include/kge_b200.h.
+// (kge_proje.cuh), of TuckER's core matrices and trunk, forward and backward (kge_tucker.cuh) and of ConvE's
+// training-mode trunk, forward and backward (kge_conve_train.cuh).  Declarations and reference citations:
+// include/kge_b200.h.
 #include <cstdlib>
 
 #include "kge_acre.cuh"
+#include "kge_conve_train.cuh"
 #include "kge_interacte.cuh"
 #include "kge_proje.cuh"
 #include "kge_tucker.cuh"
@@ -684,6 +687,132 @@ int kge_tucker_mask1(uint64_t seed, uint64_t offset, float p, int64_t Q, int32_t
   const long long n = Q * (long long)d1 * d1;
   tucker_mask1_kernel<<<proj_tiles(n, 256), 256, 0, (cudaStream_t)stream>>>(m, n, out);
   KGE_CHECK_LAUNCH("tucker_mask1_kernel");
+  return KGE_OK;
+}
+
+// ---- ConvE training-mode trunk: batch-statistics BatchNorm, dropout noise, forward and backward ----------------
+
+// KGE_OK, or the error code of an unsupported image / malformed call (message set for `fn`)
+static int conve_train_check(const kge_conve_train_t* p, const char* fn, int64_t Q, int64_t B) {
+  if (!p) { set_error("%s: null pointer", fn); return KGE_EINVAL; }
+  const int k = p->hidden_size, h1 = p->hidden_size_1;
+  if (k <= 0 || h1 < 3 || k / h1 < 2 || (k / h1) * h1 != k || 2 * k > CONVE_MAX_IMAGE) {
+    set_error("%s: unsupported image (hidden_size %d, hidden_size_1 %d)", fn, k, h1);
+    return KGE_ENOTSUP;
+  }
+  const float* ptrs[] = {p->ent, p->rel, p->bn0_weight, p->bn0_bias, p->conv_weight, p->conv_bias, p->bn1_weight,
+                         p->bn1_bias, p->fc_weight, p->fc_bias, p->bn2_weight, p->bn2_bias};
+  for (const float* t : ptrs)
+    if (!t) { set_error("%s: null parameter tensor", fn); return KGE_EINVAL; }
+  const float* run[] = {p->bn0_mean, p->bn0_var, p->bn1_mean, p->bn1_var, p->bn2_mean, p->bn2_var};
+  int nrun = 0;
+  for (const float* t : run) nrun += t != nullptr;
+  if (nrun != 0 && nrun != 6) { set_error("%s: running statistics must be all set or all NULL", fn); return KGE_EINVAL; }
+  if (B < 2 || Q < B || Q % B != 0 || (Q + PBM - 1) / PBM > 65535 || Q > 0x7fffffffll) {
+    set_error("%s: bad Q %lld / B %lld (Q a multiple of B >= 2)", fn, (long long)Q, (long long)B);
+    return KGE_EINVAL;
+  }
+  return KGE_OK;
+}
+
+static ConveTrain conve_train_args(const kge_conve_train_t* p, const int64_t* e, const int64_t* r, int64_t Q,
+                                   int64_t B, const float* noise0, const float* noise1, const float* noise2,
+                                   float* ws) {
+  ConveTrain a{};
+  a.ent = p->ent; a.rel = p->rel; a.e = e; a.r = r;
+  a.k = p->hidden_size; a.h1 = p->hidden_size_1; a.h2 = a.k / a.h1; a.Q = Q; a.B = B;
+  a.bn0_w = p->bn0_weight; a.bn0_b = p->bn0_bias; a.conv_w = p->conv_weight; a.conv_b = p->conv_bias;
+  a.bn1_w = p->bn1_weight; a.bn1_b = p->bn1_bias; a.bn2_w = p->bn2_weight; a.bn2_b = p->bn2_bias;
+  a.noise0 = noise0; a.noise1 = noise1; a.noise2 = noise2;
+  const ConveTrainLayout L = conve_train_layout(Q, B, a.k, a.h1);
+  a.img = ws + L.img; a.z1 = ws + L.z1; a.feat = ws + L.feat; a.hpre = ws + L.hpre;
+  a.st0 = ws + L.st0; a.st1 = ws + L.st1; a.st2 = ws + L.st2; a.part0 = ws + L.part0; a.part1 = ws + L.part1;
+  a.red0 = ws + L.red0; a.red1 = ws + L.red1; a.dz = ws + L.dz; a.dimg = ws + L.dimg; a.pw = ws + L.pw;
+  a.pb = ws + L.pb;
+  return a;
+}
+
+int64_t kge_conve_train_workspace_bytes(const kge_conve_train_t* p, int64_t Q, int64_t B) {
+  if (!p || p->hidden_size_1 < 3 || p->hidden_size / p->hidden_size_1 < 2 || B < 1) return 0;
+  const long long q = Q > B ? Q : B;
+  return conve_train_layout(q, B, p->hidden_size, p->hidden_size_1).total * (int64_t)sizeof(float);
+}
+
+int kge_conve_train_fwd(const kge_conve_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                        const float* noise0, const float* noise1, const float* noise2, float* x, void* workspace,
+                        int64_t workspace_bytes, void* stream) {
+  if (int rc = conve_train_check(p, "kge_conve_train_fwd", Q, B)) return rc;
+  if (!e || !r || !x || !workspace) { set_error("kge_conve_train_fwd: null pointer"); return KGE_EINVAL; }
+  if (workspace_bytes < kge_conve_train_workspace_bytes(p, Q, B)) {
+    set_error("kge_conve_train_fwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  const ConveTrain a = conve_train_args(p, e, r, Q, B, noise0, noise1, noise2, ws);
+  const int k = a.k, plane = (2 * a.h2 - 2) * (a.h1 - 2);
+  const long long F = conve_feat_width(a.h2, a.h1);
+  conve_tr_gather_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("conve_tr_gather_kernel");
+  conve_tr_bn_stats_kernel<<<1, 256, 0, st>>>(a.part0, Q, B, 1, (float)(2 * k), p->bn0_eps, p->bn0_momentum, a.st0,
+                                              p->bn0_mean, p->bn0_var);
+  KGE_CHECK_LAUNCH("conve_tr_bn_stats_kernel<bn0>");
+  conve_tr_conv_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("conve_tr_conv_kernel");
+  conve_tr_bn_stats_kernel<<<1, 256, 0, st>>>(a.part1, Q, B, CONVE_CH, (float)plane, p->bn1_eps, p->bn1_momentum,
+                                              a.st1, p->bn1_mean, p->bn1_var);
+  KGE_CHECK_LAUNCH("conve_tr_bn_stats_kernel<bn1>");
+  conve_tr_feat_kernel<<<proj_tiles(Q * F, 256), 256, 0, st>>>(a, F, plane);
+  KGE_CHECK_LAUNCH("conve_tr_feat_kernel");
+  float* partial = ws + conve_train_layout(Q, B, k, a.h1).partial;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_fc(a.feat, p->fc_weight, Q, F, k, partial), st,
+                                      "proj_gemm_kernel<conve train fc>")) return rc;
+  conve_tr_fc_combine_kernel<<<proj_tiles(Q * k, 256), 256, 0, st>>>(partial, conve_fc_slices(F), Q * k, k, p->fc_bias,
+                                                                    noise2, a.hpre);
+  KGE_CHECK_LAUNCH("conve_tr_fc_combine_kernel");
+  conve_tr_bn2_kernel<<<proj_tiles(k, 256), 256, 0, st>>>(a, p->bn2_eps, p->bn2_momentum, p->bn2_mean, p->bn2_var, x);
+  KGE_CHECK_LAUNCH("conve_tr_bn2_kernel");
+  return KGE_OK;
+}
+
+int kge_conve_train_bwd(const kge_conve_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                        const float* noise0, const float* noise1, const float* noise2, const float* gx,
+                        const float* x, float* const* grads, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (int rc = conve_train_check(p, "kge_conve_train_bwd", Q, B)) return rc;
+  if (!e || !r || !gx || !x || !grads || !workspace) { set_error("kge_conve_train_bwd: null pointer"); return KGE_EINVAL; }
+  for (int i = 0; i < KGE_CONVE_TRAIN_GRADS; ++i)
+    if (!grads[i]) { set_error("kge_conve_train_bwd: null gradient buffer %d", i); return KGE_EINVAL; }
+  if (workspace_bytes < kge_conve_train_workspace_bytes(p, Q, B)) {
+    set_error("kge_conve_train_bwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  const ConveTrain a = conve_train_args(p, e, r, Q, B, noise0, noise1, noise2, ws);
+  const int k = a.k;
+  const long long F = conve_feat_width(a.h2, a.h1);
+  float* dh = ws + conve_train_layout(Q, B, k, a.h1).dh;
+  // grads: ent, rel, bn0.w, bn0.b, conv.w, conv.b, bn1.w, bn1.b, fc.w, fc.b, bn2.w, bn2.b
+  conve_tr_bn2_bwd_kernel<<<proj_tiles(k, 256), 256, 0, st>>>(a, gx, x, dh, grads[10], grads[11], grads[9]);
+  KGE_CHECK_LAUNCH("conve_tr_bn2_bwd_kernel");
+  if (int rc = launch_gemm<EPI_ATOMIC>(conve_plan_grad_fc_w(dh, a.feat, Q, F, k, grads[8]), st,
+                                       "proj_gemm_kernel<conve grad fc_w>")) return rc;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_grad_feat(dh, p->fc_weight, Q, F, k, a.dz), st,
+                                      "proj_gemm_kernel<conve grad feat>")) return rc;
+  conve_tr_bn1_bwd_part_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("conve_tr_bn1_bwd_part_kernel");
+  conve_tr_reduce_kernel<<<1, 256, 0, st>>>(a.part1, Q, B, CONVE_CH, a.red1, grads[6], grads[7]);
+  KGE_CHECK_LAUNCH("conve_tr_reduce_kernel<bn1>");
+  conve_tr_conv_bwd_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("conve_tr_conv_bwd_kernel");
+  conve_tr_colsum_kernel<<<proj_tiles(CONVE_TAPS, 256), 256, 0, st>>>(a.pw, Q, CONVE_TAPS, grads[4]);
+  KGE_CHECK_LAUNCH("conve_tr_colsum_kernel<conv weight>");
+  conve_tr_colsum_kernel<<<1, 256, 0, st>>>(a.pb, Q, CONVE_CH, grads[5]);
+  KGE_CHECK_LAUNCH("conve_tr_colsum_kernel<conv bias>");
+  conve_tr_reduce_kernel<<<1, 256, 0, st>>>(a.part0, Q, B, 1, a.red0, grads[2], grads[3]);
+  KGE_CHECK_LAUNCH("conve_tr_reduce_kernel<bn0>");
+  conve_tr_bn0_bwd_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a, grads[0], grads[1]);
+  KGE_CHECK_LAUNCH("conve_tr_bn0_bwd_kernel");
   return KGE_OK;
 }
 

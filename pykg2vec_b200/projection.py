@@ -9,9 +9,12 @@ batches of queries with kge_proj_rank (counts only, no [Q, N] matrix, no sort).
 
 The trunk in front of it (BatchNorm -> 3x3 conv -> BatchNorm -> ReLU -> Linear -> BatchNorm ->
 ReLU on a [b, 1, 2*h2, h1] image) runs in two ways:
-  * training (autograd needed, BatchNorm batch statistics): the reference's own torch layers,
-    with TF32 convolutions disabled in forward and backward so the trunk stays fp32 like the
-    reference's CPU path;
+  * training (BatchNorm batch statistics, dropout): ConveTrunkFunction over kge_conve_train_fwd / _bwd —
+    statistics reduced in a fixed order, the running statistics updated in place, dropout as explicit
+    noise tensors drawn from torch's generator — or the Trainer's fused step on the same kernels.  The
+    reference's torch layers stay as _trunk_layers (TF32 convolutions disabled in forward and backward so
+    they stay fp32 like the reference's CPU path): the tests' yardstick, and the path for CPU tables,
+    images the kernels refuse and kge_trunk = False;
   * evaluation (`proj_query`, used by the batched Evaluator): kge_conve_trunk_fwd — gather +
     BN0 + conv + BN1 + ReLU in one kernel and the Linear layer through the same tiled GEMM as the
     tail.
@@ -86,10 +89,38 @@ def _conv2d_fp32(conv, x):
     return _Fp32Conv2d.apply(x, conv.weight, conv.bias, conv.stride, conv.padding, conv.dilation, conv.groups)
 
 
+class ConveTrunkFunction(torch.autograd.Function):
+    """x = ConvE's trunk in training mode (projection.py:86-99) on kge_conve_train_fwd; backward runs
+    kge_conve_train_bwd.  The Q = G * B rows are G groups of B rows, each with its own batch statistics; the forward
+    updates the model's running statistics in place (num_batches_tracked is the caller's).  noise0 / noise1 /
+    noise2: the dropout noise [Q, 2k] / [Q, 32] / [Q, k], or None.  params: ConvE.kge_conve_params()."""
+
+    @staticmethod
+    def forward(ctx, model, e, r, B, noise0, noise1, noise2, *params):
+        _require_cuda(e, r, *params)
+        params = [t.detach() for t in params]
+        e, r = e.contiguous(), r.contiguous()
+        x, ws = _lib.conve_train_fwd(model, e, r, B, noise0, noise1, noise2, params=params)
+        ctx.model, ctx.B, ctx.noise = model, B, (noise0, noise1, noise2)
+        ctx.save_for_backward(e, r, x, ws, *params)
+        return x
+
+    @staticmethod
+    def backward(ctx, gx):
+        e, r, x, ws, *params = ctx.saved_tensors
+        grads = [torch.zeros_like(t) for t in params]
+        _lib.conve_train_bwd(ctx.model, e, r, ctx.B, gx.contiguous(), x, grads, ws, *ctx.noise, params=params)
+        return (None,) * 7 + tuple(g if need else None for g, need in zip(grads, ctx.needs_input_grad[7:]))
+
+
 class ConvE(ProjectionModel):
     """pykg2vec/models/projection.py:12-125 — same kwargs, sub-module names (state_dict keys
     ent_embeddings / rel_embeddings / b / bn0 / conv2d_1 / bn1 / fc / bn2), parameter_list and
-    loss binding."""
+    loss binding.
+
+    In training mode with the tables on a CUDA device the trunk is ConveTrunkFunction (kge_conve_train_*); the
+    reference's torch layers stay as _trunk_layers: the yardstick of the tests, the path for CPU tables, for images
+    the kernels refuse (2k > 4096) and, with the attribute / kwarg kge_trunk = False, for everything."""
 
     def __init__(self, **kwargs):
         super(ConvE, self).__init__(self.__class__.__name__.lower())
@@ -113,12 +144,67 @@ class ConvE(ProjectionModel):
         self.bn2 = nn.BatchNorm1d(k)
         self.parameter_list = [self.ent_embeddings, self.rel_embeddings, self.b]
         self.loss = Criterion.multi_class_bce
+        self.kge_trunk = bool(kwargs.get("kge_trunk", True))
 
     def embed(self, h, r, t):
         return self.ent_embeddings(h), self.rel_embeddings(r), self.ent_embeddings(t)
 
     def embed2(self, e, r):
         return self.ent_embeddings(e), self.rel_embeddings(r)
+
+    def _kernel_trunk(self):
+        """the kernels are selected and the tables live on a CUDA device (the kernels read device memory only)"""
+        return self.kge_trunk and self.ent_embeddings.weight.is_cuda
+
+    def kge_train_supported(self):
+        """kge_conve_train_* runs this model's training trunk: kernels selected, an image they take (as
+        kge_conve_trunk_fwd: hidden_size_1 >= 3, hidden_size_2 >= 2, 2k <= 4096) and BatchNorms with running
+        statistics and a momentum"""
+        k, h1 = int(self.hidden_size), int(self.hidden_size_1)
+        bns = (self.bn0, self.bn1, self.bn2)
+        return self._kernel_trunk() and h1 >= 3 and k % h1 == 0 and k // h1 >= 2 and 2 * k <= 4096 and \
+            all(bn.track_running_stats and bn.momentum is not None for bn in bns)
+
+    def kge_conve_params(self):
+        """the 12 trunk tensors in parameters() order without the bias row b (kge_conve_train_bwd's gradient order)"""
+        return [self.ent_embeddings.weight, self.rel_embeddings.weight, self.bn0.weight, self.bn0.bias,
+                self.conv2d_1.weight, self.conv2d_1.bias, self.bn1.weight, self.bn1.bias, self.fc.weight,
+                self.fc.bias, self.bn2.weight, self.bn2.bias]
+
+    def dropout_noise(self, rows):
+        """(noise0 [rows, 2k], noise1 [rows, 32], noise2 [rows, k]) of inp_drop, feat_drop (Dropout2d: one value per
+        channel) and hidden_drop in training mode, drawn in that order as ATen draws bernoulli noise: each None when
+        its p is 0 or in eval mode, zeros when p >= 1"""
+        w = self.ent_embeddings.weight
+        out = []
+        for drop, width in ((self.inp_drop, 2 * self.hidden_size), (self.feat_drop, 32), (self.hidden_drop,
+                                                                                           self.hidden_size)):
+            p = float(drop.p)
+            if p == 0.0 or not self.training:
+                out.append(None)
+            elif p >= 1.0:
+                out.append(torch.zeros((rows, width), dtype=torch.float32, device=w.device))
+            else:
+                out.append(torch.empty((rows, width), dtype=torch.float32, device=w.device).bernoulli_(1 - p)
+                           .div_(1 - p))
+        return tuple(out)
+
+    def note_batch_stats(self, forwards=1):
+        """num_batches_tracked += forwards on the three BatchNorms (kge_conve_train_fwd updates the rest)"""
+        for bn in (self.bn0, self.bn1, self.bn2):
+            bn.num_batches_tracked.add_(forwards)
+
+    def _train_trunk(self, e, r):
+        """the training-mode trunk: ConveTrunkFunction where the kernels take it, else the torch layers"""
+        B = e.shape[0]
+        if B == 0 or not self.kge_train_supported():
+            return self._trunk_layers(e, r)
+        if B == 1:   # nn.BatchNorm1d's refusal (bn2), before anything runs
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % (torch.Size([1, int(self.hidden_size)]),))
+        x = ConveTrunkFunction.apply(self, e, r, B, *self.dropout_noise(B), *self.kge_conve_params())
+        self.note_batch_stats()
+        return x
 
     # ---- trunk: everything of inner_forward before the x . E^T product (projection.py:88-99) ----
     def _trunk_layers(self, e, r):
@@ -149,15 +235,19 @@ class ConvE(ProjectionModel):
         r = self._rel_ids(r, direction)
         if not self.training and not torch.is_grad_enabled():
             return _lib.conve_trunk_fwd(self, e.contiguous(), r.contiguous())
-        return self._trunk_layers(e, r)
+        return self._train_trunk(e, r) if self.training else self._trunk_layers(e, r)
 
     def proj_tail_tables(self):
         """(entity table [N,k], bias row [N]) of the tail product."""
         return self.ent_embeddings.weight, self.b.weight.view(-1)
 
     def forward(self, e, r, direction="tail"):
-        x = self._trunk_layers(e, self._rel_ids(r, direction)) if (self.training or torch.is_grad_enabled()) \
-            else self.proj_query(e, r, direction)
+        if self.training:
+            x = self._train_trunk(e, self._rel_ids(r, direction))
+        elif torch.is_grad_enabled():
+            x = self._trunk_layers(e, self._rel_ids(r, direction))
+        else:
+            x = self.proj_query(e, r, direction)
         return ProjTailFunction.apply(x, self.ent_embeddings.weight, self.b.weight)
 
     def predict_tail_rank(self, e, r, topk=-1):
