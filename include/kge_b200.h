@@ -458,6 +458,52 @@ int64_t kge_hyper_trunk_workspace_bytes(const kge_hyper_t* p, int64_t Q);
 int kge_hyper_trunk_fwd(const kge_hyper_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
                         void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- HypER trunk, training mode ------------------------------------------------------------
+ * HypER.forward up to the x.E^T product (pykg2vec/models/projection.py:581-606) with self.training == True, forward
+ * and backward; replaces the reference's torch layers bn0 -> inp_drop -> fc1 -> grouped conv -> bn1 ->
+ * feature_map_drop -> fc -> hidden_drop -> bn2 -> relu and their autograd.  Per query q (no ReLU after bn1):
+ *   w = fc1(rel[r[q]]) [32][9];  v = bn0(ent[e[q]]) * noise0;  z1[c][j] = sum_{t<9} w[c][t] v[j+t] (j < de-8);
+ *   x[q,:] = relu(bn2((fc(flatten(bn1(z1) * noise1)) * noise2)))
+ * The Q = G * B rows are G groups of B rows (G = 2: the tail and head forwards of train_step_projection as one call);
+ * every BatchNorm uses the batch statistics of its own group, and the running statistics are updated group after
+ * group as G sequential nn.BatchNorm calls do (momentum from the struct, unbiased variance); num_batches_tracked is
+ * the caller's.  Running-statistic pointers: all six set, or all NULL (no update).  A filter has the same bits as
+ * kge_hyper_trunk_fwd's filter of that relation.
+ * Dropout is explicit noise, bernoulli(1 - p) / (1 - p) as torch draws it (each may be NULL = no dropout):
+ *   noise0 [Q, de] (inp_drop), noise1 [Q, 32] (feature_map_drop, Dropout2d: one value per channel), noise2 [Q, de].
+ * ent_padding_idx / rel_padding_idx: the embeddings' padding_idx (-1: none); that row receives no lookup gradient
+ * (nn.Embedding's rule), its value is read as any other.
+ * Widths: 9 <= de <= 4096 (KGE_ENOTSUP beyond, as kge_hyper_trunk_fwd); B >= 2 (a one-row BatchNorm1d raises in the
+ * reference) and Q a multiple of B, else KGE_EINVAL.
+ *
+ * kge_hyper_train_fwd: x [Q, de].  Every statistic is reduced in a fixed order that does not depend on the grid, so x
+ * and the running statistics are bit-reproducible.  The workspace (kge_hyper_train_workspace_bytes(p, Q, B) bytes)
+ * keeps what the backward reads: pass the same workspace, unmodified, to kge_hyper_train_bwd.
+ * kge_hyper_train_bwd: from gx = d loss / d x [Q, de] and the forward's x, ACCUMULATES into KGE_HYPER_TRAIN_GRADS dense
+ * buffers shaped like the parameters (caller zeroes; none may be NULL), in this order: ent, rel, bn0.weight,
+ * bn0.bias, bn1.weight, bn1.bias, fc.weight, fc.bias, bn2.weight, bn2.bias, fc1.weight, fc1.bias.  The entity /
+ * relation rows are scattered with float atomics (ids repeat); every other sum runs in a fixed order.  No entry point
+ * allocates. */
+#define KGE_HYPER_TRAIN_GRADS 12
+typedef struct kge_hyper_train {
+  int32_t ent_hidden_size, rel_hidden_size;
+  int64_t ent_padding_idx, rel_padding_idx;
+  float bn0_eps, bn1_eps, bn2_eps;
+  float bn0_momentum, bn1_momentum, bn2_momentum;
+  const float* ent; const float* rel;
+  const float* bn0_weight; const float* bn0_bias; const float* bn1_weight; const float* bn1_bias;
+  const float* fc_weight; const float* fc_bias; const float* bn2_weight; const float* bn2_bias;
+  const float* fc1_weight; const float* fc1_bias;
+  float* bn0_mean; float* bn0_var; float* bn1_mean; float* bn1_var; float* bn2_mean; float* bn2_var;
+} kge_hyper_train_t;
+int64_t kge_hyper_train_workspace_bytes(const kge_hyper_train_t* p, int64_t Q, int64_t B);
+int kge_hyper_train_fwd(const kge_hyper_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                        const float* noise0, const float* noise1, const float* noise2, float* x, void* workspace,
+                        int64_t workspace_bytes, void* stream);
+int kge_hyper_train_bwd(const kge_hyper_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                        const float* noise0, const float* noise1, const float* noise2, const float* gx,
+                        const float* x, float* const* grads, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- InteractE trunk, inference mode -------------------------------------------------------
  * InteractE.forward up to the x.E^T product (pykg2vec/models/projection.py:425-442) with
  * self.training == False: dropouts are identities and bn0 / bn1 / bn2 use their running statistics.

@@ -39,6 +39,7 @@ EXPORTS = [
     "kge_tucker_workspace_bytes", "kge_tucker_cores", "kge_tucker_trunk_fwd", "kge_tucker_trunk_bwd",
     "kge_tucker_cores_bwd", "kge_tucker_mask1",
     "kge_conve_train_workspace_bytes", "kge_conve_train_fwd", "kge_conve_train_bwd",
+    "kge_hyper_train_workspace_bytes", "kge_hyper_train_fwd", "kge_hyper_train_bwd",
     "kge_project_entities", "kge_normalize_rows_to",
 ]
 
@@ -86,6 +87,7 @@ def lib():
     L.kge_acre_trunk_workspace_bytes.restype = ctypes.c_int64
     L.kge_tucker_workspace_bytes.restype = ctypes.c_int64
     L.kge_conve_train_workspace_bytes.restype = ctypes.c_int64
+    L.kge_hyper_train_workspace_bytes.restype = ctypes.c_int64
     if L.kge_abi_version() != ABI_VERSION:
         raise KgeError("libkge_b200.so ABI %d != binding ABI %d" % (L.kge_abi_version(), ABI_VERSION))
     missing = [name for name in EXPORTS if not hasattr(L, name)]
@@ -1067,6 +1069,88 @@ def conve_train_bwd(model, e, r, B, gx, x, grads, workspace, noise0=None, noise1
     check(lib().kge_conve_train_bwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0, n1,
                                     n2, _ptr(gx), _ptr(x), arr, _ptr(workspace), ctypes.c_int64(workspace.numel()),
                                     _stream()), "kge_conve_train_bwd")
+
+
+# ---- HypER training-mode trunk (include/kge_b200.h: kge_hyper_train_*) ------------------------------------------
+HYPER_TRAIN_PARAMS = ("ent", "rel", "bn0_weight", "bn0_bias", "bn1_weight", "bn1_bias", "fc_weight", "fc_bias",
+                      "bn2_weight", "bn2_bias", "fc1_weight", "fc1_bias")   # = the gradient order of kge_hyper_train_bwd
+HYPER_TRAIN_RUNNING = CONVE_TRAIN_RUNNING
+
+
+class KgeHyperTrain(ctypes.Structure):
+    """kge_hyper_train_t of include/kge_b200.h."""
+    _fields_ = [("ent_hidden_size", ctypes.c_int32), ("rel_hidden_size", ctypes.c_int32),
+                ("ent_padding_idx", ctypes.c_int64), ("rel_padding_idx", ctypes.c_int64)] + \
+               [(n, ctypes.c_float) for n in ("bn0_eps", "bn1_eps", "bn2_eps", "bn0_momentum", "bn1_momentum",
+                                              "bn2_momentum")] + \
+               [(n, ctypes.c_void_p) for n in HYPER_TRAIN_PARAMS + HYPER_TRAIN_RUNNING]
+
+
+def hyper_train_struct(model, params=None, running=True):
+    """kge_hyper_train_t of a HypER (the reference's sub-module names).  params: the 12 tensors of HYPER_TRAIN_PARAMS
+    (default: model.kge_hyper_params()); running=False leaves the running statistics alone (NULL pointers)."""
+    if params is None:
+        params = model.kge_hyper_params()
+    if len(params) != len(HYPER_TRAIN_PARAMS):
+        raise KgeError("HypER's training trunk needs its %d parameter tensors" % len(HYPER_TRAIN_PARAMS))
+    p = KgeHyperTrain()
+    p.ent_hidden_size, p.rel_hidden_size = int(model.ent_hidden_size), int(model.rel_hidden_size)
+    pads = (model.ent_embeddings.padding_idx, model.rel_embeddings.padding_idx)
+    p.ent_padding_idx, p.rel_padding_idx = (-1 if i is None else int(i) for i in pads)
+    bns = (model.bn0, model.bn1, model.bn2)
+    p.bn0_eps, p.bn1_eps, p.bn2_eps = (float(bn.eps) for bn in bns)
+    if any(bn.momentum is None for bn in bns):   # cumulative averaging: the torch layers' job
+        raise KgeNotSupported("kge_hyper_train: BatchNorm momentum None is not supported")
+    p.bn0_momentum, p.bn1_momentum, p.bn2_momentum = (float(bn.momentum) for bn in bns)
+    for name, t in zip(HYPER_TRAIN_PARAMS, params):
+        setattr(p, name, _dev_f32(t.detach(), name).data_ptr())
+    if running:
+        for i, bn in enumerate(bns):
+            setattr(p, "bn%d_mean" % i, _dev_f32(bn.running_mean, "running_mean").data_ptr())
+            setattr(p, "bn%d_var" % i, _dev_f32(bn.running_var, "running_var").data_ptr())
+    return p
+
+
+def hyper_train_fwd(model, e, r, B, noise0=None, noise1=None, noise2=None, params=None, running=True):
+    """HypER's trunk in training mode (projection.py:581-606) on Q = G * B rows, G groups of B with their own batch
+    statistics -> (x [Q, de], workspace).  Updates the model's running statistics in place (group after group) unless
+    running=False; num_batches_tracked is the caller's.  Keep the workspace for hyper_train_bwd."""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    if r.numel() != Q:
+        raise KgeError("e and r must have equal length")
+    p = hyper_train_struct(model, params, running)
+    de = p.ent_hidden_size
+    n0 = _conve_train_noise(noise0, Q, de, "noise0")
+    n1 = _conve_train_noise(noise1, Q, 32, "noise1")
+    n2 = _conve_train_noise(noise2, Q, de, "noise2")
+    nbytes = int(lib().kge_hyper_train_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q), ctypes.c_int64(B)))
+    ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=e.device)
+    x = torch.empty((Q, de), dtype=torch.float32, device=e.device)
+    check(lib().kge_hyper_train_fwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0, n1,
+                                    n2, _ptr(x), _ptr(ws), ctypes.c_int64(ws.numel()), _stream()),
+          "kge_hyper_train_fwd")
+    return x, ws
+
+
+def hyper_train_bwd(model, e, r, B, gx, x, grads, workspace, noise0=None, noise1=None, noise2=None, params=None):
+    """backward of hyper_train_fwd: accumulates into grads, 12 buffers shaped like HYPER_TRAIN_PARAMS"""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    p = hyper_train_struct(model, params, running=False)
+    params = params if params is not None else model.kge_hyper_params()
+    de = p.ent_hidden_size
+    if _dev_f32(gx, "gx").numel() != Q * de or _dev_f32(x, "x").numel() != Q * de:
+        raise KgeError("gx and x must be [Q, de]")
+    if len(grads) != len(HYPER_TRAIN_PARAMS) or any(_dev_f32(g, "grad").shape != w.shape for g, w in zip(grads, params)):
+        raise KgeError("grads must be %d buffers shaped like the parameters" % len(HYPER_TRAIN_PARAMS))
+    n0 = _conve_train_noise(noise0, Q, de, "noise0")
+    n1 = _conve_train_noise(noise1, Q, 32, "noise1")
+    n2 = _conve_train_noise(noise2, Q, de, "noise2")
+    arr = (ctypes.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
+    check(lib().kge_hyper_train_bwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0, n1,
+                                    n2, _ptr(gx), _ptr(x), arr, _ptr(workspace), ctypes.c_int64(workspace.numel()),
+                                    _stream()), "kge_hyper_train_bwd")
 
 
 def launch_count():

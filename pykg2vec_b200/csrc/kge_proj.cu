@@ -2,13 +2,14 @@
 // kge_proj.cuh), of the ConvE, HypER, InteractE and AcrE inference trunks (kge_conve.cuh, kge_hyper.cuh,
 // kge_interacte.cuh, kge_acre.cuh, which reuse the same tiled GEMM — one translation unit so the kernel
 // template is instantiated once), of ProjE_pointwise's trunk, training step and L1 regulariser
-// (kge_proje.cuh), of TuckER's core matrices and trunk, forward and backward (kge_tucker.cuh) and of ConvE's
-// training-mode trunk, forward and backward (kge_conve_train.cuh).  Declarations and reference citations:
-// include/kge_b200.h.
+// (kge_proje.cuh), of TuckER's core matrices and trunk, forward and backward (kge_tucker.cuh) and of ConvE's and
+// HypER's training-mode trunks, forward and backward (kge_conve_train.cuh, kge_hyper_train.cuh).  Declarations and
+// reference citations: include/kge_b200.h.
 #include <cstdlib>
 
 #include "kge_acre.cuh"
 #include "kge_conve_train.cuh"
+#include "kge_hyper_train.cuh"
 #include "kge_interacte.cuh"
 #include "kge_proje.cuh"
 #include "kge_tucker.cuh"
@@ -813,6 +814,144 @@ int kge_conve_train_bwd(const kge_conve_train_t* p, const int64_t* e, const int6
   KGE_CHECK_LAUNCH("conve_tr_reduce_kernel<bn0>");
   conve_tr_bn0_bwd_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a, grads[0], grads[1]);
   KGE_CHECK_LAUNCH("conve_tr_bn0_bwd_kernel");
+  return KGE_OK;
+}
+
+// ---- HypER training-mode trunk: relation-generated filters, batch-statistics BatchNorm, forward and backward ------
+
+// KGE_OK, or the error code of an unsupported width / malformed call (message set for `fn`)
+static int hyper_train_check(const kge_hyper_train_t* p, const char* fn, int64_t Q, int64_t B) {
+  if (!p) { set_error("%s: null pointer", fn); return KGE_EINVAL; }
+  const int de = p->ent_hidden_size, dr = p->rel_hidden_size;
+  if (de < HYPER_FW || de > HYPER_MAX_DE) {
+    set_error("%s: unsupported ent_hidden_size %d (needs %d <= de <= %d)", fn, de, HYPER_FW, HYPER_MAX_DE);
+    return KGE_ENOTSUP;
+  }
+  if (dr <= 0 || dr > (1 << 20)) { set_error("%s: bad rel_hidden_size %d", fn, dr); return KGE_EINVAL; }
+  const float* ptrs[] = {p->ent, p->rel, p->bn0_weight, p->bn0_bias, p->bn1_weight, p->bn1_bias, p->fc_weight,
+                         p->fc_bias, p->bn2_weight, p->bn2_bias, p->fc1_weight, p->fc1_bias};
+  for (const float* t : ptrs)
+    if (!t) { set_error("%s: null parameter tensor", fn); return KGE_EINVAL; }
+  const float* run[] = {p->bn0_mean, p->bn0_var, p->bn1_mean, p->bn1_var, p->bn2_mean, p->bn2_var};
+  int nrun = 0;
+  for (const float* t : run) nrun += t != nullptr;
+  if (nrun != 0 && nrun != 6) { set_error("%s: running statistics must be all set or all NULL", fn); return KGE_EINVAL; }
+  if (B < 2 || Q < B || Q % B != 0 || (Q + PBM - 1) / PBM > 65535 || Q > 0x7fffffffll) {
+    set_error("%s: bad Q %lld / B %lld (Q a multiple of B >= 2)", fn, (long long)Q, (long long)B);
+    return KGE_EINVAL;
+  }
+  return KGE_OK;
+}
+
+static HyperTrain hyper_train_args(const kge_hyper_train_t* p, const int64_t* e, const int64_t* r, int64_t Q,
+                                   int64_t B, const float* noise0, const float* noise1, const float* noise2,
+                                   float* ws) {
+  HyperTrain a{};
+  a.ent = p->ent; a.e = e; a.r = r;
+  a.de = p->ent_hidden_size; a.dr = p->rel_hidden_size; a.Q = Q; a.B = B;
+  a.ent_pad = p->ent_padding_idx; a.rel_pad = p->rel_padding_idx;
+  a.bn0_w = p->bn0_weight; a.bn0_b = p->bn0_bias; a.bn1_w = p->bn1_weight; a.bn1_b = p->bn1_bias;
+  a.bn2_w = p->bn2_weight; a.bn2_b = p->bn2_bias;
+  a.noise0 = noise0; a.noise1 = noise1; a.noise2 = noise2;
+  const HyperTrainLayout L = hyper_train_layout(Q, B, a.de, a.dr);
+  a.relr = ws + L.relr; a.filt = ws + L.filt; a.img = ws + L.img; a.z1 = ws + L.z1; a.feat = ws + L.feat;
+  a.hpre = ws + L.hpre; a.st0 = ws + L.st0; a.st1 = ws + L.st1; a.st2 = ws + L.st2; a.part0 = ws + L.part0;
+  a.part1 = ws + L.part1; a.red0 = ws + L.red0; a.red1 = ws + L.red1; a.dh = ws + L.dh; a.dz = ws + L.dz;
+  a.dimg = ws + L.dimg; a.dw = ws + L.dw; a.drel = ws + L.drel;
+  return a;
+}
+
+int64_t kge_hyper_train_workspace_bytes(const kge_hyper_train_t* p, int64_t Q, int64_t B) {
+  if (!p || p->ent_hidden_size < HYPER_FW || p->ent_hidden_size > HYPER_MAX_DE || p->rel_hidden_size <= 0 || B < 1)
+    return 0;
+  const long long q = Q > B ? Q : B;
+  return hyper_train_layout(q, B, p->ent_hidden_size, p->rel_hidden_size).total * (int64_t)sizeof(float);
+}
+
+int kge_hyper_train_fwd(const kge_hyper_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                        const float* noise0, const float* noise1, const float* noise2, float* x, void* workspace,
+                        int64_t workspace_bytes, void* stream) {
+  if (int rc = hyper_train_check(p, "kge_hyper_train_fwd", Q, B)) return rc;
+  if (!e || !r || !x || !workspace) { set_error("kge_hyper_train_fwd: null pointer"); return KGE_EINVAL; }
+  if (workspace_bytes < kge_hyper_train_workspace_bytes(p, Q, B)) {
+    set_error("kge_hyper_train_fwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  const HyperTrain a = hyper_train_args(p, e, r, Q, B, noise0, noise1, noise2, ws);
+  const int de = a.de, dr = a.dr, Wo = de - HYPER_FW + 1;
+  const long long F = hyper_feat_width(de);
+  tucker_gather_rows_kernel<<<proj_tiles(Q * dr, 256), 256, 0, st>>>(p->rel, r, Q, dr, a.relr);
+  KGE_CHECK_LAUNCH("tucker_gather_rows_kernel<hyper rel>");
+  if (int rc = launch_gemm<EPI_STORE>(hyper_plan_filters(a.relr, p->fc1_weight, p->fc1_bias, Q, dr, a.filt), st,
+                                      "proj_gemm_kernel<hyper train filters>")) return rc;
+  hyper_tr_gather_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("hyper_tr_gather_kernel");
+  conve_tr_bn_stats_kernel<<<1, 256, 0, st>>>(a.part0, Q, B, 1, (float)de, p->bn0_eps, p->bn0_momentum, a.st0,
+                                              p->bn0_mean, p->bn0_var);
+  KGE_CHECK_LAUNCH("conve_tr_bn_stats_kernel<hyper bn0>");
+  hyper_tr_conv_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("hyper_tr_conv_kernel");
+  conve_tr_bn_stats_kernel<<<1, 256, 0, st>>>(a.part1, Q, B, HYPER_CH, (float)Wo, p->bn1_eps, p->bn1_momentum,
+                                              a.st1, p->bn1_mean, p->bn1_var);
+  KGE_CHECK_LAUNCH("conve_tr_bn_stats_kernel<hyper bn1>");
+  hyper_tr_feat_kernel<<<proj_tiles(Q * F, 256), 256, 0, st>>>(a, F, Wo);
+  KGE_CHECK_LAUNCH("hyper_tr_feat_kernel");
+  float* partial = ws + hyper_train_layout(Q, B, de, dr).partial;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_fc(a.feat, p->fc_weight, Q, F, de, partial), st,
+                                      "proj_gemm_kernel<hyper train fc>")) return rc;
+  conve_tr_fc_combine_kernel<<<proj_tiles(Q * de, 256), 256, 0, st>>>(partial, conve_fc_slices(F), Q * de, de,
+                                                                     p->fc_bias, noise2, a.hpre);
+  KGE_CHECK_LAUNCH("conve_tr_fc_combine_kernel<hyper>");
+  conve_tr_bn2_kernel<<<proj_tiles(de, 256), 256, 0, st>>>(hyper_tr_bn2_view(a), p->bn2_eps, p->bn2_momentum,
+                                                           p->bn2_mean, p->bn2_var, x);
+  KGE_CHECK_LAUNCH("conve_tr_bn2_kernel<hyper>");
+  return KGE_OK;
+}
+
+int kge_hyper_train_bwd(const kge_hyper_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                        const float* noise0, const float* noise1, const float* noise2, const float* gx,
+                        const float* x, float* const* grads, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (int rc = hyper_train_check(p, "kge_hyper_train_bwd", Q, B)) return rc;
+  if (!e || !r || !gx || !x || !grads || !workspace) { set_error("kge_hyper_train_bwd: null pointer"); return KGE_EINVAL; }
+  for (int i = 0; i < KGE_HYPER_TRAIN_GRADS; ++i)
+    if (!grads[i]) { set_error("kge_hyper_train_bwd: null gradient buffer %d", i); return KGE_EINVAL; }
+  if (workspace_bytes < kge_hyper_train_workspace_bytes(p, Q, B)) {
+    set_error("kge_hyper_train_bwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  const HyperTrain a = hyper_train_args(p, e, r, Q, B, noise0, noise1, noise2, ws);
+  const int de = a.de, dr = a.dr;
+  const long long F = hyper_feat_width(de);
+  // grads: ent, rel, bn0.w, bn0.b, bn1.w, bn1.b, fc.w, fc.b, bn2.w, bn2.b, fc1.w, fc1.b
+  conve_tr_bn2_bwd_kernel<<<proj_tiles(de, 256), 256, 0, st>>>(hyper_tr_bn2_view(a), gx, x, a.dh, grads[8], grads[9],
+                                                               grads[7]);
+  KGE_CHECK_LAUNCH("conve_tr_bn2_bwd_kernel<hyper>");
+  if (int rc = launch_gemm<EPI_ATOMIC>(conve_plan_grad_fc_w(a.dh, a.feat, Q, F, de, grads[6]), st,
+                                       "proj_gemm_kernel<hyper grad fc_w>")) return rc;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_grad_feat(a.dh, p->fc_weight, Q, F, de, a.dz), st,
+                                      "proj_gemm_kernel<hyper grad feat>")) return rc;
+  hyper_tr_bn1_bwd_part_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("hyper_tr_bn1_bwd_part_kernel");
+  conve_tr_reduce_kernel<<<1, 256, 0, st>>>(a.part1, Q, B, HYPER_CH, a.red1, grads[4], grads[5]);
+  KGE_CHECK_LAUNCH("conve_tr_reduce_kernel<hyper bn1>");
+  hyper_tr_conv_bwd_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("hyper_tr_conv_bwd_kernel");
+  conve_tr_reduce_kernel<<<1, 256, 0, st>>>(a.part0, Q, B, 1, a.red0, grads[2], grads[3]);
+  KGE_CHECK_LAUNCH("conve_tr_reduce_kernel<hyper bn0>");
+  hyper_tr_bn0_bwd_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a, grads[0]);
+  KGE_CHECK_LAUNCH("hyper_tr_bn0_bwd_kernel");
+  if (int rc = launch_gemm<EPI_ATOMIC>(conve_plan_grad_fc_w(a.dw, a.relr, Q, dr, HYPER_FILT, grads[10]), st,
+                                       "proj_gemm_kernel<hyper grad fc1_w>")) return rc;
+  conve_tr_colsum_kernel<<<proj_tiles(HYPER_FILT, 256), 256, 0, st>>>(a.dw, Q, HYPER_FILT, grads[11]);
+  KGE_CHECK_LAUNCH("conve_tr_colsum_kernel<hyper fc1 bias>");
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_grad_feat(a.dw, p->fc1_weight, Q, dr, HYPER_FILT, a.drel), st,
+                                      "proj_gemm_kernel<hyper grad rel>")) return rc;
+  hyper_tr_scatter_rel_kernel<<<proj_tiles(Q * dr, 256), 256, 0, st>>>(a.drel, r, Q, dr, a.rel_pad, grads[1]);
+  KGE_CHECK_LAUNCH("hyper_tr_scatter_rel_kernel");
   return KGE_OK;
 }
 

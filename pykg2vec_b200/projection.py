@@ -21,9 +21,13 @@ ReLU on a [b, 1, 2*h2, h1] image) runs in two ways:
 
 HypER (projection.py:508-618) has the same tail and loss; its trunk convolves the BatchNormed entity
 row with 32 filters of width 9 that a Linear layer (fc1) generates from the query's relation.  Training
-runs the reference's layers (the per-query filters as one grouped convolution, TF32 off); evaluation
-without autograd runs kge_hyper_trunk_fwd — one GEMM for every relation's filters, one kernel for
-gather + bn0 + conv + bn1, the Linear layer on the tail's tiled GEMM, then bn2 + ReLU.
+with CUDA tables runs HyperTrunkFunction over kge_hyper_train_fwd / _bwd (the queries' filters on the tiled
+GEMM, batch statistics reduced in a fixed order, dropout as explicit noise tensors) or the Trainer's fused
+step on the same kernels; the reference's layers (the per-query filters as one grouped convolution, TF32
+off) stay as _trunk_layers for CPU tables, widths the kernels refuse, BatchNorms without a momentum or
+running statistics, and kge_trunk = False.  Evaluation without autograd runs kge_hyper_trunk_fwd — one GEMM
+for every relation's filters, one kernel for gather + bn0 + conv + bn1, the Linear layer on the tail's tiled
+GEMM, then bn2 + ReLU.
 
 InteractE (projection.py:347-505) has the same tail and loss; its trunk stacks P chequer-permuted images of the
 entity and relation features and convolves them circularly with one shared filter bank.  Training runs the
@@ -585,11 +589,40 @@ class InteractE(ProjectionModel):
         return rank
 
 
+class HyperTrunkFunction(torch.autograd.Function):
+    """x = HypER's trunk in training mode (projection.py:581-606) on kge_hyper_train_fwd; backward runs
+    kge_hyper_train_bwd.  The Q = G * B rows are G groups of B rows, each with its own batch statistics; the forward
+    updates the model's running statistics in place (num_batches_tracked is the caller's).  noise0 / noise1 / noise2:
+    the dropout noise [Q, de] / [Q, 32] / [Q, de], or None.  params: HypER.kge_hyper_params()."""
+
+    @staticmethod
+    def forward(ctx, model, e, r, B, noise0, noise1, noise2, *params):
+        _require_cuda(e, r, *params)
+        params = [t.detach() for t in params]
+        e, r = e.contiguous(), r.contiguous()
+        x, ws = _lib.hyper_train_fwd(model, e, r, B, noise0, noise1, noise2, params=params)
+        ctx.model, ctx.B, ctx.noise = model, B, (noise0, noise1, noise2)
+        ctx.save_for_backward(e, r, x, ws, *params)
+        return x
+
+    @staticmethod
+    def backward(ctx, gx):
+        e, r, x, ws, *params = ctx.saved_tensors
+        grads = [torch.zeros_like(t) for t in params]
+        _lib.hyper_train_bwd(ctx.model, e, r, ctx.B, gx.contiguous(), x, grads, ws, *ctx.noise, params=params)
+        return (None,) * 7 + tuple(g if need else None for g, need in zip(grads, ctx.needs_input_grad[7:]))
+
+
 class HypER(ProjectionModel):
     """pykg2vec/models/projection.py:508-618 — same kwargs (including the required `device`), sub-module
     names (state_dict keys b / ent_embeddings / rel_embeddings / bn0 / bn1 / bn2 / fc / fc1, padding_idx=0 on
     both embeddings), parameter_list and loss binding.  As in the reference `direction` is validated and
-    otherwise ignored: the head direction runs the same function on (t, r)."""
+    otherwise ignored: the head direction runs the same function on (t, r).
+
+    In training mode with the tables on a CUDA device the trunk is HyperTrunkFunction (kge_hyper_train_*); the
+    reference's torch layers stay as _trunk_layers: the yardstick of the tests, the path for CPU tables, for widths
+    the kernels refuse (de < 9 or de > 4096), for BatchNorms with momentum None or without running statistics and,
+    with the attribute / kwarg kge_trunk = False, for everything."""
 
     def __init__(self, **kwargs):
         super(HypER, self).__init__(self.__class__.__name__.lower())
@@ -616,12 +649,66 @@ class HypER(ProjectionModel):
         nn.init.xavier_uniform_(self.rel_embeddings.weight.data)
         self.parameter_list = [self.ent_embeddings, self.rel_embeddings]
         self.loss = Criterion.multi_class_bce
+        self.kge_trunk = bool(kwargs.get("kge_trunk", True))
 
     def embed(self, h, r, t):
         return self.ent_embeddings(h), self.rel_embeddings(r), self.ent_embeddings(t)
 
     def embed2(self, e, r):
         return self.ent_embeddings(e), self.rel_embeddings(r)
+
+    def _kernel_trunk(self):
+        """the kernels are selected and the tables live on a CUDA device (the kernels read device memory only)"""
+        return self.kge_trunk and self.ent_embeddings.weight.is_cuda
+
+    def kge_train_supported(self):
+        """kge_hyper_train_* runs this model's training trunk: kernels selected, a width they take (as
+        kge_hyper_trunk_fwd: 9 <= de <= 4096) and BatchNorms with running statistics and a momentum"""
+        bns = (self.bn0, self.bn1, self.bn2)
+        return self._kernel_trunk() and 9 <= int(self.ent_hidden_size) <= 4096 and \
+            all(bn.track_running_stats and bn.momentum is not None for bn in bns)
+
+    def kge_hyper_params(self):
+        """the 12 trunk tensors in kge_hyper_train_bwd's gradient order (parameters() without the bias row b, bn2
+        after fc)"""
+        return [self.ent_embeddings.weight, self.rel_embeddings.weight, self.bn0.weight, self.bn0.bias,
+                self.bn1.weight, self.bn1.bias, self.fc.weight, self.fc.bias, self.bn2.weight, self.bn2.bias,
+                self.fc1.weight, self.fc1.bias]
+
+    def dropout_noise(self, rows):
+        """(noise0 [rows, de], noise1 [rows, 32], noise2 [rows, de]) of inp_drop, feature_map_drop (Dropout2d: one
+        value per channel) and hidden_drop in training mode, drawn in that order as ATen draws bernoulli noise: each
+        None when its p is 0 or in eval mode, zeros when p >= 1"""
+        w = self.ent_embeddings.weight
+        de = int(self.ent_hidden_size)
+        out = []
+        for drop, width in ((self.inp_drop, de), (self.feature_map_drop, self.out_channels), (self.hidden_drop, de)):
+            p = float(drop.p)
+            if p == 0.0 or not self.training:
+                out.append(None)
+            elif p >= 1.0:
+                out.append(torch.zeros((rows, width), dtype=torch.float32, device=w.device))
+            else:
+                out.append(torch.empty((rows, width), dtype=torch.float32, device=w.device).bernoulli_(1 - p)
+                           .div_(1 - p))
+        return tuple(out)
+
+    def note_batch_stats(self, forwards=1):
+        """num_batches_tracked += forwards on the three BatchNorms (kge_hyper_train_fwd updates the rest)"""
+        for bn in (self.bn0, self.bn1, self.bn2):
+            bn.num_batches_tracked.add_(forwards)
+
+    def _train_trunk(self, e, r):
+        """the training-mode trunk: HyperTrunkFunction where the kernels take it, else the torch layers"""
+        B = e.shape[0]
+        if B == 0 or not self.kge_train_supported():
+            return self._trunk_layers(e, r)
+        if B == 1:   # nn.BatchNorm1d's refusal (bn2), before anything runs
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % (torch.Size([1, int(self.ent_hidden_size)]),))
+        x = HyperTrunkFunction.apply(self, e, r, B, *self.dropout_noise(B), *self.kge_hyper_params())
+        self.note_batch_stats()
+        return x
 
     # ---- trunk: HypER.forward before the x . E^T product (projection.py:583-606) ----
     def _trunk_layers(self, e, r):
@@ -653,7 +740,7 @@ class HypER(ProjectionModel):
         _require_cuda(e, r, self.ent_embeddings.weight)
         if not self.training and not torch.is_grad_enabled():
             return _lib.hyper_trunk_fwd(self, e.contiguous(), r.contiguous())
-        return self._trunk_layers(e, r)
+        return self._train_trunk(e, r) if self.training else self._trunk_layers(e, r)
 
     def proj_tail_tables(self):
         """(entity table [N,de], bias row [N]) of the tail product."""

@@ -22,6 +22,8 @@ Two execution modes for the same step semantics:
                              tail + BCE -> kge_tucker_trunk_bwd -> kge_tucker_cores_bwd -> kge_optim_apply_dense
       ConvE                : kge_conve_train_fwd (both directions, per-direction batch statistics) -> tail + BCE ->
                              kge_conve_train_bwd -> kge_optim_apply_dense over all 13 parameter tensors
+      HypER                : kge_hyper_train_fwd (both directions, per-direction batch statistics) -> tail + BCE ->
+                             kge_hyper_train_bwd -> kge_optim_apply_dense over all 13 parameter tensors
   * data-parallel (torch.distributed world > 1, tables replicated; SURVEY.md 8e row 3): config.dp_mode
       "grads": every rank scores ITS batch shard forward + backward into the dense gradient buffers,
                ONE all-reduce per table sums (hinge) / averages (mean-type losses) them over NVLink, then
@@ -63,6 +65,7 @@ class Trainer:
         self._proje = False
         self._tucker = False
         self._conve = False
+        self._hyper = False
 
     def build_model(self):
         """trainer.py:103-144 (optimizer selection; unknown names raise NotImplementedError)."""
@@ -107,6 +110,13 @@ class Trainer:
         self._conve = name in ("sgd", "adagrad", "adam") and getattr(self.config, "fused_step", True) and \
             self.model.model_name.lower() == "conve" and self.model.kge_train_supported()
         if self._conve:
+            params = list(self.model.parameters())
+            self._grad_scratch = [torch.zeros_like(t) for t in params]
+            self._state = [torch.zeros_like(t) for t in params] if name in ("adagrad", "adam") else None
+            self._state2 = [torch.zeros_like(t) for t in params] if name == "adam" else None
+        self._hyper = name in ("sgd", "adagrad", "adam") and getattr(self.config, "fused_step", True) and \
+            self.model.model_name.lower() == "hyper" and self.model.kge_train_supported()
+        if self._hyper:
             params = list(self.model.parameters())
             self._grad_scratch = [torch.zeros_like(t) for t in params]
             self._state = [torch.zeros_like(t) for t in params] if name in ("adagrad", "adam") else None
@@ -388,6 +398,50 @@ class Trainer:
                                    self._state2[k] if self._state2 else None, step=self._step)
         return loss
 
+    def _fused_hyper(self, ids):
+        """HypER: train_step_projection (trainer.py:159-174) + backward + optimizer.step() without an autograd graph.
+        Both directions run as ONE trunk launch sequence over 2B rows (HypER has no reciprocal relations: both use r),
+        each direction with its own batch statistics and the running statistics updated tail first; then the shared
+        tail, the BCE loss and its gradient per direction, the tail's backward, the trunk's, and one dense optimizer
+        sweep over every parameter tensor (all 13 get a gradient every step, as under loss.backward())."""
+        h, r, t, hr_t, tr_h = ids
+        m = self.model
+        B = r.numel()
+        if B == 1:   # nn.BatchNorm1d's refusal (bn2), before anything runs
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % (torch.Size([1, int(m.ent_hidden_size)]),))
+        plist = list(m.parameters())   # b, ent, rel, bn0.*, bn1.*, bn2.*, fc.*, fc1.*
+        at = {id(w): i for i, w in enumerate(plist)}
+        order = [at[id(w)] for w in m.kge_hyper_params()]
+        params = [w.detach() for w in plist]
+        trunk = [params[i] for i in order]
+        ent, bias = m.ent_embeddings.weight.detach(), m.b.detach()
+        e2, r2 = torch.cat([h, t]), torch.cat([r, r])   # rows [0, B): tail direction, [B, 2B): head
+        nt, nh = m.dropout_noise(B), m.dropout_noise(B)   # the reference's draw order: tail forward, then head
+        noise = [None if a is None else torch.cat([a, b]) for a, b in zip(nt, nh)]
+        x, ws = _lib.hyper_train_fwd(m, e2, r2, B, *noise, params=trunk)
+        m.note_batch_stats(2)
+        preds = _lib.proj_tail_fwd(x, ent, bias)
+        scale, shift = 1.0, 0.0
+        if hasattr(self.config, "label_smoothing"):
+            scale, shift = 1.0 - self.config.label_smoothing, 1.0 / self.config.tot_entity
+        grads = self._grad_scratch
+        gent, gb = grads[at[id(m.ent_embeddings.weight)]], grads[at[id(m.b)]]
+        gx = torch.zeros_like(x)
+        loss = None
+        for lo, lab in ((0, hr_t), (B, tr_h)):
+            part, gp = _lib.proj_bce(preds[lo:lo + B], lab.to(torch.float32).contiguous(), scale, shift)
+            _lib.proj_tail_bwd(gp, preds[lo:lo + B], x[lo:lo + B], ent, gx[lo:lo + B], gent, gb)
+            loss = part if loss is None else loss + part
+        del preds, gp
+        _lib.hyper_train_bwd(m, e2, r2, B, gx, x, [grads[i] for i in order], ws, *noise, params=trunk)
+        self._step += 1
+        lr = float(self.config.learning_rate)
+        for k, w in enumerate(params):
+            _lib.optim_apply_dense(w, grads[k], self._opt_code(), lr, self._state[k] if self._state else None,
+                                   self._state2[k] if self._state2 else None, step=self._step)
+        return loss
+
     # ---- one batch, host ids in, host loss out (trainer.py:269-300) -----------------------------
     def _to_device(self, arrays):
         """Pack the batch's id arrays into one pinned staging buffer and issue ONE H2D copy
@@ -490,6 +544,9 @@ class Trainer:
         if self._conve:
             with torch.no_grad():
                 return self._fused_conve(ids)
+        if self._hyper:
+            with torch.no_grad():
+                return self._fused_hyper(ids)
         if self._fused:
             with torch.no_grad():
                 if strategy == TrainingStrategy.PAIRWISE_BASED:
@@ -540,7 +597,7 @@ class Trainer:
         else:
             ids, nbytes = self._to_device(list(data))
         self.last_h2d_bytes = nbytes
-        if self._fused or self._proje or self._tucker or self._conve:
+        if self._fused or self._proje or self._tucker or self._conve or self._hyper:
             loss = self.train_batch_device(ids)
             if not sync:
                 return loss                # device tensor; float(loss) syncs when the caller wants the value
