@@ -540,6 +540,60 @@ int64_t kge_interacte_trunk_workspace_bytes(const kge_interacte_t* p, int64_t Q)
 int kge_interacte_trunk_fwd(const kge_interacte_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
                             void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- InteractE trunk, training mode ---------------------------------------------------------
+ * InteractE.forward up to the x.E^T product (pykg2vec/models/projection.py:425-442) with self.training == True,
+ * forward and backward; replaces the reference's torch layers bn0 -> inp_drop -> circular conv -> bn1 -> relu ->
+ * feature_map_drop -> fc -> hidden_drop -> bn2 -> relu and their autograd.  Geometry and per-query function as
+ * kge_interacte_trunk_fwd (H = 2*reshape_width, W = reshape_height, HW = H*W = 2k, pad = ks/2, C1 = P*F):
+ *   img[p] = comb[perm[p]] viewed [H][W];  v[p] = bn0_p(img[p]) * noise0[q, p, :, :]
+ *   z1[p*F+f][i][j] = sum_{u,v<ks} conv_filt[f][u][v] * v[p][(i+u-pad) mod H][(j+v-pad) mod W]   (no bias)
+ *   x[q,:] = relu(bn2((fc(flatten(relu(bn1(z1)) * noise1[q, c]))) * noise2[q, :]))
+ * The Q = G * B rows are G groups of B rows (G = 2: the tail and head forwards of train_step_projection as one call);
+ * every BatchNorm uses the batch statistics of its own group (bn0 per image channel p over B*HW values, bn1 per
+ * channel over B*HW, bn2 per feature over B), and the running statistics are updated group after group as G
+ * sequential nn.BatchNorm calls do (momentum from the struct, unbiased variance); num_batches_tracked is the
+ * caller's.  Running-statistic pointers: all six set, or all NULL (no update).  perm: int64 [P, 2k] on the device,
+ * every row a permutation of 0 .. 2k-1 (the backward's un-permute relies on it; not checked here).
+ * Dropout is explicit noise, bernoulli(1 - p) / (1 - p) as torch draws it (each may be NULL = no dropout):
+ *   noise0 [Q, P*2k] (inp_drop on [Q, P, H, W]), noise1 [Q, C1] (feature_map_drop, Dropout2d: one value per
+ *   channel), noise2 [Q, k] (hidden_drop).  The embeddings have no padding_idx.
+ * Shapes: the bounds of kge_interacte_trunk_fwd (odd ks >= 3, pad <= min(H, W), filter bank + bn1 folds + P padded
+ * images within 227 KB of shared memory; KGE_ENOTSUP beyond); B >= 2 (a one-row BatchNorm1d raises in the reference)
+ * and Q a multiple of B, else KGE_EINVAL.
+ *
+ * kge_interacte_train_fwd: x [Q, k].  Every statistic is reduced in a fixed order that does not depend on the grid,
+ * so x and the running statistics are bit-reproducible.  The workspace (kge_interacte_train_workspace_bytes(p, Q, B)
+ * bytes) keeps what the backward reads: pass the same workspace, unmodified, to kge_interacte_train_bwd, once (the
+ * backward overwrites the forward's feature maps with their gradient).  It holds two [Q, P*F*H*W] arrays (z1 and
+ * feat / d feat), the Linear layer's slice partials [ceil(P*F*H*W / 512), Q, k], the per-query d conv_filt
+ * [Q, F*ks*ks] and O(Q * (P*HW + k)) more: ~103 MB at (1, 96, 9, 20x10) with Q = 256, ~250 MB at (4, 64, 7).  The
+ * statistics span the group, so the call cannot be split over Q.
+ * kge_interacte_train_bwd: from gx = d loss / d x [Q, k] and the forward's x, ACCUMULATES into
+ * KGE_INTERACTE_TRAIN_GRADS dense buffers shaped like the parameters (caller zeroes; none may be NULL), in this order:
+ * ent, rel, bn0.weight, bn0.bias, conv_filt, bn1.weight, bn1.bias, fc.weight, fc.bias, bn2.weight, bn2.bias.  The
+ * entity / relation rows are scattered with float atomics (ids repeat); every other sum runs in a fixed order.  No
+ * entry point allocates. */
+#define KGE_INTERACTE_TRAIN_GRADS 11
+typedef struct kge_interacte_train {
+  int32_t feature_permutation, num_filters, kernel_size, reshape_height, reshape_width;
+  float bn0_eps, bn1_eps, bn2_eps;
+  float bn0_momentum, bn1_momentum, bn2_momentum;
+  const int64_t* perm;
+  const float* ent; const float* rel;
+  const float* bn0_weight; const float* bn0_bias; const float* conv_filt;
+  const float* bn1_weight; const float* bn1_bias; const float* fc_weight; const float* fc_bias;
+  const float* bn2_weight; const float* bn2_bias;
+  float* bn0_mean; float* bn0_var; float* bn1_mean; float* bn1_var; float* bn2_mean; float* bn2_var;
+} kge_interacte_train_t;
+int64_t kge_interacte_train_workspace_bytes(const kge_interacte_train_t* p, int64_t Q, int64_t B);
+int kge_interacte_train_fwd(const kge_interacte_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                            const float* noise0, const float* noise1, const float* noise2, float* x, void* workspace,
+                            int64_t workspace_bytes, void* stream);
+int kge_interacte_train_bwd(const kge_interacte_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                            const float* noise0, const float* noise1, const float* noise2, const float* gx,
+                            const float* x, float* const* grads, void* workspace, int64_t workspace_bytes,
+                            void* stream);
+
 /* ---- AcrE trunk, inference mode ------------------------------------------------------------
  * AcrE.forward up to the x.E^T product (pykg2vec/models/projection.py:706-734) with self.training == False:
  * dropouts are identities and bn0 / bn1 / bn2 use their running statistics.  C = in_channels, conv l is a

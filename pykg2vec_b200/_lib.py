@@ -40,6 +40,7 @@ EXPORTS = [
     "kge_tucker_cores_bwd", "kge_tucker_mask1",
     "kge_conve_train_workspace_bytes", "kge_conve_train_fwd", "kge_conve_train_bwd",
     "kge_hyper_train_workspace_bytes", "kge_hyper_train_fwd", "kge_hyper_train_bwd",
+    "kge_interacte_train_workspace_bytes", "kge_interacte_train_fwd", "kge_interacte_train_bwd",
     "kge_project_entities", "kge_normalize_rows_to",
 ]
 
@@ -88,6 +89,7 @@ def lib():
     L.kge_tucker_workspace_bytes.restype = ctypes.c_int64
     L.kge_conve_train_workspace_bytes.restype = ctypes.c_int64
     L.kge_hyper_train_workspace_bytes.restype = ctypes.c_int64
+    L.kge_interacte_train_workspace_bytes.restype = ctypes.c_int64
     if L.kge_abi_version() != ABI_VERSION:
         raise KgeError("libkge_b200.so ABI %d != binding ABI %d" % (L.kge_abi_version(), ABI_VERSION))
     missing = [name for name in EXPORTS if not hasattr(L, name)]
@@ -1151,6 +1153,113 @@ def hyper_train_bwd(model, e, r, B, gx, x, grads, workspace, noise0=None, noise1
     check(lib().kge_hyper_train_bwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0, n1,
                                     n2, _ptr(gx), _ptr(x), arr, _ptr(workspace), ctypes.c_int64(workspace.numel()),
                                     _stream()), "kge_hyper_train_bwd")
+
+
+# ---- InteractE training-mode trunk (include/kge_b200.h: kge_interacte_train_*) --------------------------------------
+INTERACTE_TRAIN_PARAMS = ("ent", "rel", "bn0_weight", "bn0_bias", "conv_filt", "bn1_weight", "bn1_bias", "fc_weight",
+                          "fc_bias", "bn2_weight", "bn2_bias")   # = the gradient order of kge_interacte_train_bwd
+INTERACTE_TRAIN_RUNNING = CONVE_TRAIN_RUNNING
+
+
+class KgeInteracteTrain(ctypes.Structure):
+    """kge_interacte_train_t of include/kge_b200.h."""
+    _fields_ = [(n, ctypes.c_int32) for n in ("feature_permutation", "num_filters", "kernel_size", "reshape_height",
+                                              "reshape_width")] + \
+               [(n, ctypes.c_float) for n in ("bn0_eps", "bn1_eps", "bn2_eps", "bn0_momentum", "bn1_momentum",
+                                              "bn2_momentum")] + \
+               [("perm", ctypes.c_void_p)] + \
+               [(n, ctypes.c_void_p) for n in INTERACTE_TRAIN_PARAMS + INTERACTE_TRAIN_RUNNING]
+
+
+def interacte_train_struct(model, params=None, running=True, perm=None):
+    """kge_interacte_train_t of an InteractE (the reference's sub-module names).  params: the 11 tensors of
+    INTERACTE_TRAIN_PARAMS (default: model.kge_interacte_params()); running=False leaves the running statistics alone
+    (NULL pointers); perm: the chequer permutation, int64 on the tables' device (default: model.chequer_perm)."""
+    if params is None:
+        params = model.kge_interacte_params()
+    if len(params) != len(INTERACTE_TRAIN_PARAMS):
+        raise KgeError("InteractE's training trunk needs its %d parameter tensors" % len(INTERACTE_TRAIN_PARAMS))
+    p = KgeInteracteTrain()
+    p.feature_permutation, p.num_filters, p.kernel_size = (int(model.feature_permutation), int(model.num_filters),
+                                                           int(model.kernel_size))
+    p.reshape_height, p.reshape_width = int(model.reshape_height), int(model.reshape_width)
+    bns = (model.bn0, model.bn1, model.bn2)
+    p.bn0_eps, p.bn1_eps, p.bn2_eps = (float(bn.eps) for bn in bns)
+    if any(bn.momentum is None for bn in bns):   # cumulative averaging: the torch layers' job
+        raise KgeNotSupported("kge_interacte_train: BatchNorm momentum None is not supported")
+    p.bn0_momentum, p.bn1_momentum, p.bn2_momentum = (float(bn.momentum) for bn in bns)
+    for name, t in zip(INTERACTE_TRAIN_PARAMS, params):
+        setattr(p, name, _dev_f32(t.detach(), name).data_ptr())
+    perm = model.chequer_perm if perm is None else perm
+    if perm.device != params[0].device or perm.dtype != torch.int64:
+        perm = perm.to(device=params[0].device, dtype=torch.int64)
+    p.perm = _dev_i64(perm.contiguous(), "chequer_perm").data_ptr()
+    if running:
+        for i, bn in enumerate(bns):
+            setattr(p, "bn%d_mean" % i, _dev_f32(bn.running_mean, "running_mean").data_ptr())
+            setattr(p, "bn%d_var" % i, _dev_f32(bn.running_var, "running_var").data_ptr())
+    return p, perm
+
+
+def _interacte_noise_widths(p):
+    """(noise0, noise1, noise2) row widths: P * 2k, P * F, k"""
+    k = p.reshape_height * p.reshape_width
+    return p.feature_permutation * 2 * k, p.feature_permutation * p.num_filters, k
+
+
+def interacte_train_workspace_bytes(model, Q, B):
+    """bytes of device workspace one kge_interacte_train_fwd / _bwd pair needs for Q = G * B rows (0 for a geometry
+    the kernels refuse)"""
+    p = KgeInteracteTrain()
+    p.feature_permutation, p.num_filters, p.kernel_size = (int(model.feature_permutation), int(model.num_filters),
+                                                           int(model.kernel_size))
+    p.reshape_height, p.reshape_width = int(model.reshape_height), int(model.reshape_width)
+    return int(lib().kge_interacte_train_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q), ctypes.c_int64(B)))
+
+
+def interacte_train_fwd(model, e, r, B, noise0=None, noise1=None, noise2=None, params=None, running=True, perm=None):
+    """InteractE's trunk in training mode (projection.py:425-442) on Q = G * B rows, G groups of B with their own batch
+    statistics -> (x [Q, k], workspace).  Updates the model's running statistics in place (group after group) unless
+    running=False; num_batches_tracked is the caller's.  Keep the workspace for ONE interacte_train_bwd."""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    if r.numel() != Q:
+        raise KgeError("e and r must have equal length")
+    p, perm = interacte_train_struct(model, params, running, perm)
+    w0, w1, w2 = _interacte_noise_widths(p)
+    n0 = _conve_train_noise(noise0, Q, w0, "noise0")
+    n1 = _conve_train_noise(noise1, Q, w1, "noise1")
+    n2 = _conve_train_noise(noise2, Q, w2, "noise2")
+    nbytes = int(lib().kge_interacte_train_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q), ctypes.c_int64(B)))
+    ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=e.device)
+    x = torch.empty((Q, w2), dtype=torch.float32, device=e.device)
+    check(lib().kge_interacte_train_fwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0,
+                                        n1, n2, _ptr(x), _ptr(ws), ctypes.c_int64(ws.numel()), _stream()),
+          "kge_interacte_train_fwd")
+    return x, ws
+
+
+def interacte_train_bwd(model, e, r, B, gx, x, grads, workspace, noise0=None, noise1=None, noise2=None, params=None,
+                        perm=None):
+    """backward of interacte_train_fwd: accumulates into grads, 11 buffers shaped like INTERACTE_TRAIN_PARAMS.  It
+    overwrites the forward's feature maps in the workspace: one backward per forward."""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    params = params if params is not None else model.kge_interacte_params()
+    p, perm = interacte_train_struct(model, params, False, perm)
+    w0, w1, w2 = _interacte_noise_widths(p)
+    if _dev_f32(gx, "gx").numel() != Q * w2 or _dev_f32(x, "x").numel() != Q * w2:
+        raise KgeError("gx and x must be [Q, k]")
+    if len(grads) != len(INTERACTE_TRAIN_PARAMS) or \
+            any(_dev_f32(g, "grad").shape != w.shape for g, w in zip(grads, params)):
+        raise KgeError("grads must be %d buffers shaped like the parameters" % len(INTERACTE_TRAIN_PARAMS))
+    n0 = _conve_train_noise(noise0, Q, w0, "noise0")
+    n1 = _conve_train_noise(noise1, Q, w1, "noise1")
+    n2 = _conve_train_noise(noise2, Q, w2, "noise2")
+    arr = (ctypes.c_void_p * len(grads))(*[g.data_ptr() for g in grads])
+    check(lib().kge_interacte_train_bwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0,
+                                        n1, n2, _ptr(gx), _ptr(x), arr, _ptr(workspace),
+                                        ctypes.c_int64(workspace.numel()), _stream()), "kge_interacte_train_bwd")
 
 
 def launch_count():

@@ -2,15 +2,16 @@
 // kge_proj.cuh), of the ConvE, HypER, InteractE and AcrE inference trunks (kge_conve.cuh, kge_hyper.cuh,
 // kge_interacte.cuh, kge_acre.cuh, which reuse the same tiled GEMM — one translation unit so the kernel
 // template is instantiated once), of ProjE_pointwise's trunk, training step and L1 regulariser
-// (kge_proje.cuh), of TuckER's core matrices and trunk, forward and backward (kge_tucker.cuh) and of ConvE's and
-// HypER's training-mode trunks, forward and backward (kge_conve_train.cuh, kge_hyper_train.cuh).  Declarations and
-// reference citations: include/kge_b200.h.
+// (kge_proje.cuh), of TuckER's core matrices and trunk, forward and backward (kge_tucker.cuh) and of ConvE's,
+// HypER's and InteractE's training-mode trunks, forward and backward (kge_conve_train.cuh, kge_hyper_train.cuh,
+// kge_interacte_train.cuh).  Declarations and reference citations: include/kge_b200.h.
 #include <cstdlib>
 
 #include "kge_acre.cuh"
 #include "kge_conve_train.cuh"
 #include "kge_hyper_train.cuh"
 #include "kge_interacte.cuh"
+#include "kge_interacte_train.cuh"
 #include "kge_proje.cuh"
 #include "kge_tucker.cuh"
 
@@ -952,6 +953,158 @@ int kge_hyper_train_bwd(const kge_hyper_train_t* p, const int64_t* e, const int6
                                       "proj_gemm_kernel<hyper grad rel>")) return rc;
   hyper_tr_scatter_rel_kernel<<<proj_tiles(Q * dr, 256), 256, 0, st>>>(a.drel, r, Q, dr, a.rel_pad, grads[1]);
   KGE_CHECK_LAUNCH("hyper_tr_scatter_rel_kernel");
+  return KGE_OK;
+}
+
+// ---- InteractE training-mode trunk: chequer-permuted circular convolution, batch-statistics BatchNorm -------------
+
+// KGE_OK, or the error code of an unsupported geometry / malformed call (message set for `fn`)
+static int interacte_train_check(const kge_interacte_train_t* p, const char* fn, int64_t Q, int64_t B) {
+  if (!p) { set_error("%s: null pointer", fn); return KGE_EINVAL; }
+  kge_interacte_t geo{};   // the inference trunk's shape rules
+  geo.feature_permutation = p->feature_permutation; geo.num_filters = p->num_filters;
+  geo.kernel_size = p->kernel_size; geo.reshape_height = p->reshape_height; geo.reshape_width = p->reshape_width;
+  geo.num_rel = 1;
+  if (int rc = interacte_shape(&geo, fn)) return rc;
+  const float* ptrs[] = {p->ent, p->rel, p->bn0_weight, p->bn0_bias, p->conv_filt, p->bn1_weight, p->bn1_bias,
+                         p->fc_weight, p->fc_bias, p->bn2_weight, p->bn2_bias};
+  for (const float* t : ptrs)
+    if (!t) { set_error("%s: null parameter tensor", fn); return KGE_EINVAL; }
+  if (!p->perm) { set_error("%s: null perm", fn); return KGE_EINVAL; }
+  const float* run[] = {p->bn0_mean, p->bn0_var, p->bn1_mean, p->bn1_var, p->bn2_mean, p->bn2_var};
+  int nrun = 0;
+  for (const float* t : run) nrun += t != nullptr;
+  if (nrun != 0 && nrun != 6) { set_error("%s: running statistics must be all set or all NULL", fn); return KGE_EINVAL; }
+  if (B < 2 || Q < B || Q % B != 0 || (Q + PBM - 1) / PBM > 65535 || Q > 0x7fffffffll) {
+    set_error("%s: bad Q %lld / B %lld (Q a multiple of B >= 2)", fn, (long long)Q, (long long)B);
+    return KGE_EINVAL;
+  }
+  return KGE_OK;
+}
+
+static InteracteTrainLayout interacte_train_layout_of(const kge_interacte_train_t* p, int64_t Q, int64_t B) {
+  return interacte_train_layout(Q, B, p->feature_permutation, p->num_filters, p->kernel_size, 2 * p->reshape_width,
+                                p->reshape_height);
+}
+
+static InteracteTrain interacte_train_args(const kge_interacte_train_t* p, const int64_t* e, const int64_t* r,
+                                           int64_t Q, int64_t B, const float* noise0, const float* noise1,
+                                           const float* noise2, float* ws) {
+  InteracteTrain a{};
+  a.ent = p->ent; a.rel = p->rel; a.perm = p->perm; a.e = e; a.r = r;
+  a.P = p->feature_permutation; a.F = p->num_filters; a.ks = p->kernel_size;
+  a.H = 2 * p->reshape_width; a.W = p->reshape_height; a.Q = Q; a.B = B;
+  a.bn0_w = p->bn0_weight; a.bn0_b = p->bn0_bias; a.filt = p->conv_filt; a.bn1_w = p->bn1_weight;
+  a.bn1_b = p->bn1_bias; a.bn2_w = p->bn2_weight; a.bn2_b = p->bn2_bias;
+  a.noise0 = noise0; a.noise1 = noise1; a.noise2 = noise2;
+  const InteracteTrainLayout L = interacte_train_layout_of(p, Q, B);
+  a.img = ws + L.img; a.z1 = ws + L.z1; a.feat = ws + L.feat; a.hpre = ws + L.hpre; a.st0 = ws + L.st0;
+  a.st1 = ws + L.st1; a.st2 = ws + L.st2; a.part0 = ws + L.part0; a.part1 = ws + L.part1; a.red0 = ws + L.red0;
+  a.red1 = ws + L.red1; a.dh = ws + L.dh; a.dimg = ws + L.dimg; a.pw = ws + L.pw;
+  return a;
+}
+
+// dynamic shared memory of a launch above the 48 KB default: opt the kernel in first
+static int interacte_tr_smem_optin(const void* kernel, size_t bytes) {
+  if (bytes > 48 * 1024) KGE_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  return KGE_OK;
+}
+
+int64_t kge_interacte_train_workspace_bytes(const kge_interacte_train_t* p, int64_t Q, int64_t B) {
+  if (!p || B < 1) return 0;
+  kge_interacte_t geo{};
+  geo.feature_permutation = p->feature_permutation; geo.num_filters = p->num_filters;
+  geo.kernel_size = p->kernel_size; geo.reshape_height = p->reshape_height; geo.reshape_width = p->reshape_width;
+  geo.num_rel = 1;
+  if (interacte_shape(&geo, "kge_interacte_train_workspace_bytes")) return 0;
+  return interacte_train_layout_of(p, Q > B ? Q : B, B).total * (int64_t)sizeof(float);
+}
+
+int kge_interacte_train_fwd(const kge_interacte_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                            const float* noise0, const float* noise1, const float* noise2, float* x, void* workspace,
+                            int64_t workspace_bytes, void* stream) {
+  if (int rc = interacte_train_check(p, "kge_interacte_train_fwd", Q, B)) return rc;
+  if (!e || !r || !x || !workspace) { set_error("kge_interacte_train_fwd: null pointer"); return KGE_EINVAL; }
+  if (workspace_bytes < kge_interacte_train_workspace_bytes(p, Q, B)) {
+    set_error("kge_interacte_train_fwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  const InteracteTrain a = interacte_train_args(p, e, r, Q, B, noise0, noise1, noise2, ws);
+  const int P = a.P, F = a.F, HW = a.H * a.W, k = HW / 2, C1 = P * F;
+  const long long Fw = (long long)C1 * HW;
+  interacte_tr_gather_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("interacte_tr_gather_kernel");
+  conve_tr_bn_stats_kernel<<<proj_tiles(P, 256), 256, 0, st>>>(a.part0, Q, B, P, (float)HW, p->bn0_eps,
+                                                              p->bn0_momentum, a.st0, p->bn0_mean, p->bn0_var);
+  KGE_CHECK_LAUNCH("conve_tr_bn_stats_kernel<interacte bn0>");
+  const size_t smem = (size_t)interacte_train_smem(P, F, a.ks, a.H, a.W).total * sizeof(float);
+  if (int rc = interacte_tr_smem_optin((const void*)interacte_tr_conv_kernel, smem)) return rc;
+  interacte_tr_conv_kernel<<<(unsigned)Q, CONVE_TR_THREADS, smem, st>>>(a);
+  KGE_CHECK_LAUNCH("interacte_tr_conv_kernel");
+  conve_tr_bn_stats_kernel<<<proj_tiles(C1, 256), 256, 0, st>>>(a.part1, Q, B, C1, (float)HW, p->bn1_eps,
+                                                               p->bn1_momentum, a.st1, p->bn1_mean, p->bn1_var);
+  KGE_CHECK_LAUNCH("conve_tr_bn_stats_kernel<interacte bn1>");
+  interacte_tr_feat_kernel<<<proj_tiles(Q * Fw, 256), 256, 0, st>>>(a, Fw, HW);
+  KGE_CHECK_LAUNCH("interacte_tr_feat_kernel");
+  float* partial = ws + interacte_train_layout_of(p, Q, B).partial;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_fc(a.feat, p->fc_weight, Q, Fw, k, partial), st,
+                                      "proj_gemm_kernel<interacte train fc>")) return rc;
+  conve_tr_fc_combine_kernel<<<proj_tiles(Q * k, 256), 256, 0, st>>>(partial, conve_fc_slices(Fw), Q * k, k,
+                                                                    p->fc_bias, noise2, a.hpre);
+  KGE_CHECK_LAUNCH("conve_tr_fc_combine_kernel<interacte>");
+  conve_tr_bn2_kernel<<<proj_tiles(k, 256), 256, 0, st>>>(interacte_tr_bn2_view(a), p->bn2_eps, p->bn2_momentum,
+                                                          p->bn2_mean, p->bn2_var, x);
+  KGE_CHECK_LAUNCH("conve_tr_bn2_kernel<interacte>");
+  return KGE_OK;
+}
+
+int kge_interacte_train_bwd(const kge_interacte_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                            const float* noise0, const float* noise1, const float* noise2, const float* gx,
+                            const float* x, float* const* grads, void* workspace, int64_t workspace_bytes,
+                            void* stream) {
+  if (int rc = interacte_train_check(p, "kge_interacte_train_bwd", Q, B)) return rc;
+  if (!e || !r || !gx || !x || !grads || !workspace) {
+    set_error("kge_interacte_train_bwd: null pointer");
+    return KGE_EINVAL;
+  }
+  for (int i = 0; i < KGE_INTERACTE_TRAIN_GRADS; ++i)
+    if (!grads[i]) { set_error("kge_interacte_train_bwd: null gradient buffer %d", i); return KGE_EINVAL; }
+  if (workspace_bytes < kge_interacte_train_workspace_bytes(p, Q, B)) {
+    set_error("kge_interacte_train_bwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  const InteracteTrain a = interacte_train_args(p, e, r, Q, B, noise0, noise1, noise2, ws);
+  const int P = a.P, F = a.F, HW = a.H * a.W, k = HW / 2, C1 = P * F, taps = a.ks * a.ks;
+  const long long Fw = (long long)C1 * HW;
+  // grads: ent, rel, bn0.w, bn0.b, conv_filt, bn1.w, bn1.b, fc.w, fc.b, bn2.w, bn2.b
+  conve_tr_bn2_bwd_kernel<<<proj_tiles(k, 256), 256, 0, st>>>(interacte_tr_bn2_view(a), gx, x, a.dh, grads[9],
+                                                              grads[10], grads[8]);
+  KGE_CHECK_LAUNCH("conve_tr_bn2_bwd_kernel<interacte>");
+  // d fc.weight reads feat before d feat overwrites it (same stream, in order)
+  if (int rc = launch_gemm<EPI_ATOMIC>(conve_plan_grad_fc_w(a.dh, a.feat, Q, Fw, k, grads[7]), st,
+                                       "proj_gemm_kernel<interacte grad fc_w>")) return rc;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_grad_feat(a.dh, p->fc_weight, Q, Fw, k, a.feat), st,
+                                      "proj_gemm_kernel<interacte grad feat>")) return rc;
+  interacte_tr_bn1_bwd_part_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("interacte_tr_bn1_bwd_part_kernel");
+  conve_tr_reduce_kernel<<<proj_tiles(C1, 256), 256, 0, st>>>(a.part1, Q, B, C1, a.red1, grads[5], grads[6]);
+  KGE_CHECK_LAUNCH("conve_tr_reduce_kernel<interacte bn1>");
+  const size_t smem = (size_t)interacte_train_smem(P, F, a.ks, a.H, a.W).total * sizeof(float);
+  if (int rc = interacte_tr_smem_optin((const void*)interacte_tr_conv_bwd_kernel, smem)) return rc;
+  interacte_tr_conv_bwd_kernel<<<(unsigned)Q, CONVE_TR_THREADS, smem, st>>>(a);
+  KGE_CHECK_LAUNCH("interacte_tr_conv_bwd_kernel");
+  conve_tr_colsum_kernel<<<proj_tiles(F * taps, 256), 256, 0, st>>>(a.pw, Q, F * taps, grads[4]);
+  KGE_CHECK_LAUNCH("conve_tr_colsum_kernel<interacte conv_filt>");
+  conve_tr_reduce_kernel<<<proj_tiles(P, 256), 256, 0, st>>>(a.part0, Q, B, P, a.red0, grads[2], grads[3]);
+  KGE_CHECK_LAUNCH("conve_tr_reduce_kernel<interacte bn0>");
+  const size_t ismem = (size_t)P * HW * sizeof(int);
+  if (int rc = interacte_tr_smem_optin((const void*)interacte_tr_bn0_bwd_kernel, ismem)) return rc;
+  interacte_tr_bn0_bwd_kernel<<<(unsigned)Q, CONVE_TR_THREADS, ismem, st>>>(a, grads[0], grads[1]);
+  KGE_CHECK_LAUNCH("interacte_tr_bn0_bwd_kernel");
   return KGE_OK;
 }
 

@@ -30,9 +30,14 @@ for every relation's filters, one kernel for gather + bn0 + conv + bn1, the Line
 GEMM, then bn2 + ReLU.
 
 InteractE (projection.py:347-505) has the same tail and loss; its trunk stacks P chequer-permuted images of the
-entity and relation features and convolves them circularly with one shared filter bank.  Training runs the
-reference's layers; evaluation without autograd runs kge_interacte_trunk_fwd — one kernel for gather +
-permutation + bn0 + circular conv + bn1 + ReLU, then HypER's Linear GEMM and bn2 + ReLU.
+entity and relation features and convolves them circularly with one shared filter bank.  Training with CUDA tables
+runs InteracteTrunkFunction over kge_interacte_train_fwd / _bwd (the circular conv with the filter bank in shared
+memory, batch statistics reduced in a fixed order, dropout as explicit noise tensors) or the Trainer's fused step on
+the same kernels; the reference's layers (the circular convolution through _Fp32Conv2d, TF32 off) stay as
+_trunk_layers for CPU tables, geometries the kernels refuse, BatchNorms without a momentum or running statistics, a
+chequer_perm whose rows are not permutations, and kge_trunk = False.  Evaluation without autograd runs
+kge_interacte_trunk_fwd — one kernel for gather + permutation + bn0 + circular conv + bn1 + ReLU, then HypER's
+Linear GEMM and bn2 + ReLU.
 
 AcrE (projection.py:621-746) has the same tail and loss; its trunk runs three dilated (atrous) 3x3 convolutions
 on the 20 x 20 image of the stacked entity and relation rows, chained with a residual add (serial way) or side
@@ -480,6 +485,33 @@ def _chequer_perm(hidden_size, reshape_width, P):
     return torch.from_numpy(np.stack(rows).astype(np.int64))
 
 
+class InteracteTrunkFunction(torch.autograd.Function):
+    """x = InteractE's trunk in training mode (projection.py:425-442) on kge_interacte_train_fwd; backward runs
+    kge_interacte_train_bwd.  The Q = G * B rows are G groups of B rows, each with its own batch statistics; the
+    forward updates the model's running statistics in place (num_batches_tracked is the caller's).  noise0 / noise1 /
+    noise2: the dropout noise [Q, P*2k] / [Q, P*F] / [Q, k], or None.  params: InteractE.kge_interacte_params().
+    The backward reuses the forward's feature-map buffer, so the graph is backpropagated once."""
+
+    @staticmethod
+    def forward(ctx, model, e, r, B, noise0, noise1, noise2, *params):
+        _require_cuda(e, r, *params)
+        params = [t.detach() for t in params]
+        e, r = e.contiguous(), r.contiguous()
+        perm = model._perm_on(e.device)
+        x, ws = _lib.interacte_train_fwd(model, e, r, B, noise0, noise1, noise2, params=params, perm=perm)
+        ctx.model, ctx.B, ctx.noise, ctx.perm = model, B, (noise0, noise1, noise2), perm
+        ctx.save_for_backward(e, r, x, ws, *params)
+        return x
+
+    @staticmethod
+    def backward(ctx, gx):
+        e, r, x, ws, *params = ctx.saved_tensors
+        grads = [torch.zeros_like(t) for t in params]
+        _lib.interacte_train_bwd(ctx.model, e, r, ctx.B, gx.contiguous(), x, grads, ws, *ctx.noise, params=params,
+                                 perm=ctx.perm)
+        return (None,) * 7 + tuple(g if need else None for g, need in zip(grads, ctx.needs_input_grad[7:]))
+
+
 class InteractE(ProjectionModel):
     """pykg2vec/models/projection.py:347-505 — same kwargs (including the required `device`; hidden_size is read
     and then replaced by reshape_width * reshape_height), sub-module names and state_dict keys (bias / conv_filt /
@@ -488,9 +520,13 @@ class InteractE(ProjectionModel):
     is a plain attribute: not a parameter or buffer, so not in state_dict.  As in the reference `direction` is
     validated and otherwise ignored: the head direction runs the same function on (t, r).
 
-    Training runs the reference's layers (the circular convolution through _Fp32Conv2d with TF32 off, so
-    conv_filt trains); evaluation without autograd runs kge_interacte_trunk_fwd — one kernel for gather +
-    permutation + bn0 + circular conv + bn1 + ReLU, the Linear layer on the tail's tiled GEMM, then bn2 + ReLU."""
+    In training mode with the tables on a CUDA device the trunk is InteracteTrunkFunction (kge_interacte_train_*);
+    the reference's torch layers (the circular convolution through _Fp32Conv2d with TF32 off, so conv_filt trains)
+    stay as _trunk_layers: the yardstick of the tests, the path for CPU tables, for geometries the kernels refuse, for
+    BatchNorms with momentum None or without running statistics, for a chequer_perm whose rows are not permutations
+    of 0 .. 2k-1 and, with the attribute / kwarg kge_trunk = False, for everything.  Evaluation without autograd runs
+    kge_interacte_trunk_fwd — one kernel for gather + permutation + bn0 + circular conv + bn1 + ReLU, the Linear
+    layer on the tail's tiled GEMM, then bn2 + ReLU."""
 
     def __init__(self, **kwargs):
         super(InteractE, self).__init__(self.__class__.__name__.lower())
@@ -525,6 +561,8 @@ class InteractE(ProjectionModel):
         self.parameter_list = [self.ent_embeddings, self.rel_embeddings]
         self.loss = Criterion.multi_class_bce
         self._perm_dev = None
+        self._perm_valid = None
+        self.kge_trunk = bool(kwargs.get("kge_trunk", True))
 
     def embed(self, h, r, t):
         return self.ent_embeddings(h), self.rel_embeddings(r), self.ent_embeddings(t)
@@ -541,6 +579,72 @@ class InteractE(ProjectionModel):
         if self._perm_dev is None or self._perm_dev[0] is not src or self._perm_dev[1].device != device:
             self._perm_dev = (src, src.to(device=device, dtype=torch.int64))
         return self._perm_dev[1]
+
+    def _perm_is_permutation(self):
+        """every row of chequer_perm ([P, 2k]) is a permutation of 0 .. 2k-1, which the training kernels' un-permute
+        relies on: checked once per attribute value"""
+        src = self.chequer_perm
+        if self._perm_valid is None or self._perm_valid[0] is not src:
+            n, P = 2 * int(self.hidden_size), int(self.feature_permutation)
+            ok = tuple(src.shape) == (P, n) and not src.is_floating_point() and not src.is_complex()
+            if ok:
+                want = torch.arange(n, device=src.device, dtype=torch.int64).expand(P, n)
+                ok = bool(torch.equal(torch.sort(src.to(torch.int64), dim=1).values, want))
+            self._perm_valid = (src, ok)
+        return self._perm_valid[1]
+
+    def _kernel_trunk(self):
+        """the kernels are selected and the tables live on a CUDA device (the kernels read device memory only)"""
+        return self.kge_trunk and self.ent_embeddings.weight.is_cuda
+
+    def kge_train_supported(self):
+        """kge_interacte_train_* runs this model's training trunk: kernels selected, a geometry they take (as
+        kge_interacte_trunk_fwd), BatchNorms with running statistics and a momentum, and a chequer_perm whose rows
+        are permutations"""
+        bns = (self.bn0, self.bn1, self.bn2)
+        return self._kernel_trunk() and all(bn.track_running_stats and bn.momentum is not None for bn in bns) and \
+            _lib.interacte_train_workspace_bytes(self, 2, 2) > 0 and self._perm_is_permutation()
+
+    def kge_interacte_params(self):
+        """the 11 trunk tensors in kge_interacte_train_bwd's gradient order (parameters() without the bias row)"""
+        return [self.ent_embeddings.weight, self.rel_embeddings.weight, self.bn0.weight, self.bn0.bias, self.conv_filt,
+                self.bn1.weight, self.bn1.bias, self.fc.weight, self.fc.bias, self.bn2.weight, self.bn2.bias]
+
+    def dropout_noise(self, rows):
+        """(noise0 [rows, P*2k], noise1 [rows, P*F], noise2 [rows, k]) of inp_drop (on the [rows, P, H, W] images),
+        feature_map_drop (Dropout2d: one value per channel) and hidden_drop in training mode, drawn in that order as
+        ATen draws bernoulli noise: each None when its p is 0 or in eval mode, zeros when p >= 1"""
+        w = self.ent_embeddings.weight
+        k, P = int(self.hidden_size), int(self.feature_permutation)
+        out = []
+        for drop, width in ((self.inp_drop, P * 2 * k), (self.feature_map_drop, P * int(self.num_filters)),
+                            (self.hidden_drop, k)):
+            p = float(drop.p)
+            if p == 0.0 or not self.training:
+                out.append(None)
+            elif p >= 1.0:
+                out.append(torch.zeros((rows, width), dtype=torch.float32, device=w.device))
+            else:
+                out.append(torch.empty((rows, width), dtype=torch.float32, device=w.device).bernoulli_(1 - p)
+                           .div_(1 - p))
+        return tuple(out)
+
+    def note_batch_stats(self, forwards=1):
+        """num_batches_tracked += forwards on the three BatchNorms (kge_interacte_train_fwd updates the rest)"""
+        for bn in (self.bn0, self.bn1, self.bn2):
+            bn.num_batches_tracked.add_(forwards)
+
+    def _train_trunk(self, e, r):
+        """the training-mode trunk: InteracteTrunkFunction where the kernels take it, else the torch layers"""
+        B = e.shape[0]
+        if B == 0 or not self.kge_train_supported():
+            return self._trunk_layers(e, r)
+        if B == 1:   # nn.BatchNorm1d's refusal (bn2), before anything runs
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % (torch.Size([1, int(self.hidden_size)]),))
+        x = InteracteTrunkFunction.apply(self, e, r, B, *self.dropout_noise(B), *self.kge_interacte_params())
+        self.note_batch_stats()
+        return x
 
     # ---- trunk: InteractE.forward before the x . E^T product (projection.py:427-442) ----
     def _trunk_layers(self, e, r):
@@ -571,7 +675,7 @@ class InteractE(ProjectionModel):
         _require_cuda(e, r, self.ent_embeddings.weight)
         if not self.training and not torch.is_grad_enabled():
             return _lib.interacte_trunk_fwd(self, e.contiguous(), r.contiguous(), perm=self._perm_on(e.device))
-        return self._trunk_layers(e, r)
+        return self._train_trunk(e, r) if self.training else self._trunk_layers(e, r)
 
     def proj_tail_tables(self):
         """(entity table [N,k], bias row [N]) of the tail product."""
