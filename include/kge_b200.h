@@ -636,6 +636,69 @@ int64_t kge_acre_trunk_workspace_bytes(const kge_acre_t* p, int64_t Q);
 int kge_acre_trunk_fwd(const kge_acre_t* p, const int64_t* e, const int64_t* r, int64_t Q, float* x,
                        void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- AcrE trunk, training mode ---------------------------------------------------------------
+ * AcrE.forward up to the x.E^T product (pykg2vec/models/projection.py:706-734) with self.training == True, forward
+ * and backward; replaces the reference's torch layers bn0 -> inp_drop -> three dilated convs (+ residual, or the
+ * W_gate_e mix) -> bn1 -> relu -> feature_map_drop -> fc -> hidden_drop -> bn2 -> relu and their autograd.  The
+ * configuration and per-query function are kge_acre_trunk_fwd's, with v = bn0(img) * noise0[q, :] in place of bn0(img):
+ *   serial (way 0):   y = conv3(conv2(conv1(v))) + v;   parallel (way 1): y[c] = W_gate_e([v ; conv1..3(v)[c]])
+ *   x[q,:] = relu(bn2(fc(flatten(relu(bn1(y)) * noise1[q, c])) * noise2[q, :]))
+ * The Q = G * B rows are G groups of B rows (G = 2: the tail and head forwards of train_step_projection as one call);
+ * every BatchNorm uses the batch statistics of its own group (bn0 one channel over B*400 values, bn1 per channel over
+ * B*400, bn2 per feature over B), and the running statistics are updated group after group as G sequential
+ * nn.BatchNorm calls do (momentum from the struct, unbiased variance); num_batches_tracked is the caller's.
+ * Running-statistic pointers: all six set, or all NULL (no update).  rel is indexed with r as given.
+ * Dropout is explicit noise, bernoulli(1 - p) / (1 - p) as torch draws it (each may be NULL = no dropout):
+ *   noise0 [Q, 400] (inp_drop), noise1 [Q, C] (feature_map_drop, Dropout2d: one value per channel), noise2 [Q, 200].
+ * Pointers: the shapes of kge_acre_t: ent [N,200], rel [num_rel,200], conv*_bias all three set for acre_bias or all NULL,
+ * W_gate_e_* set in the parallel way and ignored in the serial one; the running statistics are the
+ * six writable pointers at the end.
+ * KGE_EINVAL: way not 0 / 1, an atrous rate < 1, in_channels < 1, num_rel < 1, one or two NULL conv biases, a NULL
+ * required pointer, B < 2 (a one-row BatchNorm1d raises in the reference), Q not a multiple of B, or Q (parallel:
+ * Q*C) beyond one call's grid.  KGE_ENOTSUP: hidden_size != 200; a serial C whose backward's shared memory exceeds
+ * 227 KB, 4*(400 + 802*C + 9*C*ceil8(C) + ceil8(C)) bytes, so C <= 46 (the inference trunk's bound); a parallel
+ * C > 1024.  Any atrous rate >= 1 runs, including rates beyond the 20 x 20 image.
+ *
+ * kge_acre_train_fwd: x [Q, 200].  Every statistic is reduced in a fixed order that does not depend on the grid, so
+ * x and the running statistics are bit-reproducible.  The workspace (kge_acre_train_workspace_bytes(p, Q, B) bytes)
+ * keeps what the backward reads: pass the same workspace, unmodified, to kge_acre_train_bwd, once (the backward
+ * overwrites the forward's features and gate rows with their gradients).  In floats it holds
+ *   Q*(400*(2 + 2C) + 200*(ceil(400C/512) + 2) + 9*C*(Cin2 + Cin3 + 1) + 5C + 2) + G*(4*C + 404)
+ * rounded up per region to 64 floats, plus Q*800C for the serial way's conv1 / conv2 outputs or Q*1600C for the
+ * parallel way's gate rows (Cin2 = Cin3 = C serial, 1 parallel): 78 MB at (serial, 32) and 25 MB at (parallel, 9)
+ * with Q = 256, B = 128.  The statistics span the group, so the call cannot be split over Q.
+ * kge_acre_train_bwd: from gx = d loss / d x [Q, 200] and the forward's x, ACCUMULATES into KGE_ACRE_TRAIN_GRADS
+ * dense buffers shaped like the parameters (caller zeroes), in this order: ent, rel, bn0.weight, bn0.bias,
+ * conv1.weight, conv1.bias, conv2.weight, conv2.bias, conv3.weight, conv3.bias, W_gate_e.weight, W_gate_e.bias,
+ * bn1.weight, bn1.bias, fc.weight, fc.bias, bn2.weight, bn2.bias.  The slots of absent parameters (the conv biases
+ * without acre_bias, W_gate_e in the serial way) must be NULL and every other slot set, else KGE_EINVAL.  The entity /
+ * relation rows are scattered with float atomics (ids repeat); every other sum runs in a fixed order.  No entry
+ * point allocates. */
+#define KGE_ACRE_TRAIN_GRADS 18
+typedef struct kge_acre_train {
+  int32_t in_channels, way, first_atrous, second_atrous, third_atrous, hidden_size;
+  int64_t num_rel;
+  float bn0_eps, bn1_eps, bn2_eps;
+  float bn0_momentum, bn1_momentum, bn2_momentum;
+  const float* ent; const float* rel;
+  const float* bn0_weight; const float* bn0_bias;
+  const float* conv1_weight; const float* conv1_bias;
+  const float* conv2_weight; const float* conv2_bias;
+  const float* conv3_weight; const float* conv3_bias;
+  const float* W_gate_e_weight; const float* W_gate_e_bias;
+  const float* bn1_weight; const float* bn1_bias;
+  const float* fc_weight; const float* fc_bias;
+  const float* bn2_weight; const float* bn2_bias;
+  float* bn0_mean; float* bn0_var; float* bn1_mean; float* bn1_var; float* bn2_mean; float* bn2_var;
+} kge_acre_train_t;
+int64_t kge_acre_train_workspace_bytes(const kge_acre_train_t* p, int64_t Q, int64_t B);
+int kge_acre_train_fwd(const kge_acre_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                       const float* noise0, const float* noise1, const float* noise2, float* x, void* workspace,
+                       int64_t workspace_bytes, void* stream);
+int kge_acre_train_bwd(const kge_acre_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                       const float* noise0, const float* noise1, const float* noise2, const float* gx, const float* x,
+                       float* const* grads, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- ProjE_pointwise (pykg2vec/models/projection.py:128-257) ------------------------------------
  * Tables with the reference's state_dict shapes (device fp32): ent [num_ent, k], rel [num_rel, k],
  * bc1 / De1 / Dr1 / bc2 / De2 / Dr2 [1, k].  k = hidden_size <= 1024 (KGE_ENOTSUP above).

@@ -41,6 +41,7 @@ EXPORTS = [
     "kge_conve_train_workspace_bytes", "kge_conve_train_fwd", "kge_conve_train_bwd",
     "kge_hyper_train_workspace_bytes", "kge_hyper_train_fwd", "kge_hyper_train_bwd",
     "kge_interacte_train_workspace_bytes", "kge_interacte_train_fwd", "kge_interacte_train_bwd",
+    "kge_acre_train_workspace_bytes", "kge_acre_train_fwd", "kge_acre_train_bwd",
     "kge_project_entities", "kge_normalize_rows_to",
 ]
 
@@ -90,6 +91,7 @@ def lib():
     L.kge_conve_train_workspace_bytes.restype = ctypes.c_int64
     L.kge_hyper_train_workspace_bytes.restype = ctypes.c_int64
     L.kge_interacte_train_workspace_bytes.restype = ctypes.c_int64
+    L.kge_acre_train_workspace_bytes.restype = ctypes.c_int64
     if L.kge_abi_version() != ABI_VERSION:
         raise KgeError("libkge_b200.so ABI %d != binding ABI %d" % (L.kge_abi_version(), ABI_VERSION))
     missing = [name for name in EXPORTS if not hasattr(L, name)]
@@ -1260,6 +1262,118 @@ def interacte_train_bwd(model, e, r, B, gx, x, grads, workspace, noise0=None, no
     check(lib().kge_interacte_train_bwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0,
                                         n1, n2, _ptr(gx), _ptr(x), arr, _ptr(workspace),
                                         ctypes.c_int64(workspace.numel()), _stream()), "kge_interacte_train_bwd")
+
+
+# ---- AcrE training-mode trunk (include/kge_b200.h: kge_acre_train_*) ----------------------------------------------
+ACRE_TRAIN_PARAMS = ("ent", "rel", "bn0_weight", "bn0_bias", "conv1_weight", "conv1_bias", "conv2_weight",
+                     "conv2_bias", "conv3_weight", "conv3_bias", "W_gate_e_weight", "W_gate_e_bias", "bn1_weight",
+                     "bn1_bias", "fc_weight", "fc_bias", "bn2_weight", "bn2_bias")   # = kge_acre_train_bwd's slots
+ACRE_TRAIN_RUNNING = CONVE_TRAIN_RUNNING
+
+
+class KgeAcreTrain(ctypes.Structure):
+    """kge_acre_train_t of include/kge_b200.h."""
+    _fields_ = [(n, ctypes.c_int32) for n in ("in_channels", "way", "first_atrous", "second_atrous", "third_atrous",
+                                              "hidden_size")] + \
+               [("num_rel", ctypes.c_int64)] + \
+               [(n, ctypes.c_float) for n in ("bn0_eps", "bn1_eps", "bn2_eps", "bn0_momentum", "bn1_momentum",
+                                              "bn2_momentum")] + \
+               [(n, ctypes.c_void_p) for n in ACRE_TRAIN_PARAMS + ACRE_TRAIN_RUNNING]
+
+
+def acre_train_present(model):
+    """the names of ACRE_TRAIN_PARAMS this AcrE has: no conv biases without acre_bias, W_gate_e in the parallel way
+    only"""
+    par = model.way != "serial"
+    bias = model.conv1.bias is not None
+    return tuple(n for n in ACRE_TRAIN_PARAMS
+                 if not (n.startswith("conv") and n.endswith("_bias") and not bias)
+                 and not (n.startswith("W_gate_e") and not par))
+
+
+def _acre_train_config(model):
+    p = KgeAcreTrain()
+    way = "serial" if model.way == "serial" else "parallel"      # the reference's test: any other value is parallel
+    p.way = ACRE_WAYS[way]
+    p.in_channels, p.hidden_size = int(model.in_channels), int(model.ent_embeddings.weight.shape[1])
+    p.num_rel = int(model.rel_embeddings.weight.shape[0])
+    p.first_atrous, p.second_atrous, p.third_atrous = (int(model.first_atrous), int(model.second_atrous),
+                                                       int(model.third_atrous))
+    return p
+
+
+def acre_train_struct(model, params=None, running=True):
+    """kge_acre_train_t of an AcrE (the reference's sub-module names).  params: the present trunk tensors in
+    ACRE_TRAIN_PARAMS order (default: model.kge_acre_params()); running=False leaves the running statistics alone
+    (NULL pointers).  Absent parameters stay NULL."""
+    if params is None:
+        params = model.kge_acre_params()
+    names = acre_train_present(model)
+    if len(params) != len(names):
+        raise KgeError("AcrE's training trunk needs its %d parameter tensors" % len(names))
+    p = _acre_train_config(model)
+    bns = (model.bn0, model.bn1, model.bn2)
+    p.bn0_eps, p.bn1_eps, p.bn2_eps = (float(bn.eps) for bn in bns)
+    if any(bn.momentum is None for bn in bns):   # cumulative averaging: the torch layers' job
+        raise KgeNotSupported("kge_acre_train: BatchNorm momentum None is not supported")
+    p.bn0_momentum, p.bn1_momentum, p.bn2_momentum = (float(bn.momentum) for bn in bns)
+    for name, t in zip(names, params):
+        setattr(p, name, _dev_f32(t.detach(), name).data_ptr())
+    if running:
+        for i, bn in enumerate(bns):
+            setattr(p, "bn%d_mean" % i, _dev_f32(bn.running_mean, "running_mean").data_ptr())
+            setattr(p, "bn%d_var" % i, _dev_f32(bn.running_var, "running_var").data_ptr())
+    return p
+
+
+def acre_train_workspace_bytes(model, Q, B):
+    """bytes of device workspace one kge_acre_train_fwd / _bwd pair needs for Q = G * B rows (0 for a configuration
+    the kernels refuse)"""
+    p = _acre_train_config(model)
+    return int(lib().kge_acre_train_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q), ctypes.c_int64(B)))
+
+
+def acre_train_fwd(model, e, r, B, noise0=None, noise1=None, noise2=None, params=None, running=True):
+    """AcrE's trunk in training mode (projection.py:706-734) on Q = G * B rows, G groups of B with their own batch
+    statistics -> (x [Q, 200], workspace).  Updates the model's running statistics in place (group after group) unless
+    running=False; num_batches_tracked is the caller's.  Keep the workspace for ONE acre_train_bwd."""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    if r.numel() != Q:
+        raise KgeError("e and r must have equal length")
+    p = acre_train_struct(model, params, running)
+    n0 = _conve_train_noise(noise0, Q, 400, "noise0")
+    n1 = _conve_train_noise(noise1, Q, int(p.in_channels), "noise1")
+    n2 = _conve_train_noise(noise2, Q, 200, "noise2")
+    nbytes = int(lib().kge_acre_train_workspace_bytes(ctypes.byref(p), ctypes.c_int64(Q), ctypes.c_int64(B)))
+    ws = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=e.device)
+    x = torch.empty((Q, 200), dtype=torch.float32, device=e.device)
+    check(lib().kge_acre_train_fwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0, n1,
+                                   n2, _ptr(x), _ptr(ws), ctypes.c_int64(ws.numel()), _stream()), "kge_acre_train_fwd")
+    return x, ws
+
+
+def acre_train_bwd(model, e, r, B, gx, x, grads, workspace, noise0=None, noise1=None, noise2=None, params=None):
+    """backward of acre_train_fwd: accumulates into grads, one buffer shaped like each tensor of params (the present
+    parameters in ACRE_TRAIN_PARAMS order).  It overwrites the forward's features in the workspace: one backward per
+    forward."""
+    e, r = _dev_i64(e, "e"), _dev_i64(r, "r")
+    Q = e.numel()
+    params = params if params is not None else model.kge_acre_params()
+    p = acre_train_struct(model, params, False)
+    if _dev_f32(gx, "gx").numel() != Q * 200 or _dev_f32(x, "x").numel() != Q * 200:
+        raise KgeError("gx and x must be [Q, 200]")
+    if len(grads) != len(params) or any(_dev_f32(g, "grad").shape != w.shape for g, w in zip(grads, params)):
+        raise KgeError("grads must be %d buffers shaped like the parameters" % len(params))
+    n0 = _conve_train_noise(noise0, Q, 400, "noise0")
+    n1 = _conve_train_noise(noise1, Q, int(p.in_channels), "noise1")
+    n2 = _conve_train_noise(noise2, Q, 200, "noise2")
+    slots = dict(zip(acre_train_present(model), grads))
+    arr = (ctypes.c_void_p * len(ACRE_TRAIN_PARAMS))(*[slots[n].data_ptr() if n in slots else None
+                                                        for n in ACRE_TRAIN_PARAMS])
+    check(lib().kge_acre_train_bwd(ctypes.byref(p), _ptr(e), _ptr(r), ctypes.c_int64(Q), ctypes.c_int64(B), n0, n1,
+                                   n2, _ptr(gx), _ptr(x), arr, _ptr(workspace), ctypes.c_int64(workspace.numel()),
+                                   _stream()), "kge_acre_train_bwd")
 
 
 def launch_count():

@@ -3,11 +3,13 @@
 // kge_interacte.cuh, kge_acre.cuh, which reuse the same tiled GEMM — one translation unit so the kernel
 // template is instantiated once), of ProjE_pointwise's trunk, training step and L1 regulariser
 // (kge_proje.cuh), of TuckER's core matrices and trunk, forward and backward (kge_tucker.cuh) and of ConvE's,
-// HypER's and InteractE's training-mode trunks, forward and backward (kge_conve_train.cuh, kge_hyper_train.cuh,
-// kge_interacte_train.cuh).  Declarations and reference citations: include/kge_b200.h.
+// HypER's, InteractE's and AcrE's training-mode trunks, forward and backward (kge_conve_train.cuh,
+// kge_hyper_train.cuh, kge_interacte_train.cuh, kge_acre_train.cuh).  Declarations and reference citations:
+// include/kge_b200.h.
 #include <cstdlib>
 
 #include "kge_acre.cuh"
+#include "kge_acre_train.cuh"
 #include "kge_conve_train.cuh"
 #include "kge_hyper_train.cuh"
 #include "kge_interacte.cuh"
@@ -1105,6 +1107,234 @@ int kge_interacte_train_bwd(const kge_interacte_train_t* p, const int64_t* e, co
   if (int rc = interacte_tr_smem_optin((const void*)interacte_tr_bn0_bwd_kernel, ismem)) return rc;
   interacte_tr_bn0_bwd_kernel<<<(unsigned)Q, CONVE_TR_THREADS, ismem, st>>>(a, grads[0], grads[1]);
   KGE_CHECK_LAUNCH("interacte_tr_bn0_bwd_kernel");
+  return KGE_OK;
+}
+
+// ---- AcrE training-mode trunk: serial / parallel atrous convolutions, batch-statistics BatchNorm ------------------
+
+// KGE_OK, or the error code of an unsupported configuration (message set for `fn`); the shape rules only
+static int acre_train_shape(const kge_acre_train_t* p, const char* fn) {
+  const int C = p->in_channels;
+  if ((p->way != 0 && p->way != 1) || C < 1 || p->first_atrous < 1 || p->second_atrous < 1 || p->third_atrous < 1 ||
+      p->num_rel < 1) {
+    set_error("%s: bad configuration way=%d in_channels=%d atrous %d/%d/%d num_rel %lld", fn, p->way, C,
+              p->first_atrous, p->second_atrous, p->third_atrous, (long long)p->num_rel);
+    return KGE_EINVAL;
+  }
+  if (p->hidden_size != ACRE_K) {
+    set_error("%s: unsupported hidden_size %d (the trunk views each row as 10 x 20: needs 200)", fn, p->hidden_size);
+    return KGE_ENOTSUP;
+  }
+  if (p->way == 0 && acre_tr_serial_smem(C).total * (long long)sizeof(float) > ACRE_SMEM_MAX) {
+    set_error("%s: serial in_channels %d exceeds the shared-memory bound (C <= 46)", fn, C);
+    return KGE_ENOTSUP;
+  }
+  if (p->way == 1 && C > ACRE_TR_PAR_MAX) {
+    set_error("%s: parallel in_channels %d above %d", fn, C, ACRE_TR_PAR_MAX);
+    return KGE_ENOTSUP;
+  }
+  return KGE_OK;
+}
+
+// the 18 parameter pointers in the gradient order of kge_acre_train_bwd
+static void acre_train_ptrs(const kge_acre_train_t* p, const float* out[KGE_ACRE_TRAIN_GRADS]) {
+  const float* v[KGE_ACRE_TRAIN_GRADS] = {p->ent, p->rel, p->bn0_weight, p->bn0_bias, p->conv1_weight, p->conv1_bias,
+                                          p->conv2_weight, p->conv2_bias, p->conv3_weight, p->conv3_bias,
+                                          p->W_gate_e_weight, p->W_gate_e_bias, p->bn1_weight, p->bn1_bias,
+                                          p->fc_weight, p->fc_bias, p->bn2_weight, p->bn2_bias};
+  for (int i = 0; i < KGE_ACRE_TRAIN_GRADS; ++i) out[i] = v[i];
+}
+
+// slot i is present for this configuration: conv biases with acre_bias only, W_gate_e in the parallel way only
+static bool acre_train_present(const kge_acre_train_t* p, int i) {
+  if (i == 5 || i == 7 || i == 9) return p->conv1_bias != nullptr;
+  if (i == 10 || i == 11) return p->way == 1;
+  return true;
+}
+
+// KGE_OK, or the error code of an unsupported geometry / malformed call (message set for `fn`)
+static int acre_train_check(const kge_acre_train_t* p, const char* fn, int64_t Q, int64_t B) {
+  if (!p) { set_error("%s: null pointer", fn); return KGE_EINVAL; }
+  if (int rc = acre_train_shape(p, fn)) return rc;
+  const int nbias = (p->conv1_bias != nullptr) + (p->conv2_bias != nullptr) + (p->conv3_bias != nullptr);
+  if (nbias != 0 && nbias != 3) {
+    set_error("%s: conv biases must be all set (acre_bias) or all NULL", fn);
+    return KGE_EINVAL;
+  }
+  const float* ptrs[KGE_ACRE_TRAIN_GRADS];
+  acre_train_ptrs(p, ptrs);
+  for (int i = 0; i < KGE_ACRE_TRAIN_GRADS; ++i)
+    if (acre_train_present(p, i) && !ptrs[i]) { set_error("%s: null parameter tensor %d", fn, i); return KGE_EINVAL; }
+  const float* run[] = {p->bn0_mean, p->bn0_var, p->bn1_mean, p->bn1_var, p->bn2_mean, p->bn2_var};
+  int nrun = 0;
+  for (const float* t : run) nrun += t != nullptr;
+  if (nrun != 0 && nrun != 6) { set_error("%s: running statistics must be all set or all NULL", fn); return KGE_EINVAL; }
+  const long long rows = p->way == 1 ? Q * p->in_channels : Q;
+  if (B < 2 || Q < B || Q % B != 0 || Q > 0x7fffffffll || (rows + PBM - 1) / PBM > 65535) {
+    set_error("%s: bad Q %lld / B %lld (Q a multiple of B >= 2)", fn, (long long)Q, (long long)B);
+    return KGE_EINVAL;
+  }
+  return KGE_OK;
+}
+
+static AcreTrain acre_train_args(const kge_acre_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                                 const float* noise0, const float* noise1, float* ws) {
+  AcreTrain a{};
+  a.ent = p->ent; a.rel = p->rel; a.e = e; a.r = r;
+  a.C = p->in_channels; a.dil[0] = p->first_atrous; a.dil[1] = p->second_atrous; a.dil[2] = p->third_atrous;
+  a.par = p->way == 1; a.has_bias = p->conv1_bias != nullptr; a.Q = Q; a.B = B;
+  a.bn0_w = p->bn0_weight; a.bn0_b = p->bn0_bias;
+  a.conv_w[0] = p->conv1_weight; a.conv_w[1] = p->conv2_weight; a.conv_w[2] = p->conv3_weight;
+  a.conv_b[0] = p->conv1_bias; a.conv_b[1] = p->conv2_bias; a.conv_b[2] = p->conv3_bias;
+  a.bn1_w = p->bn1_weight; a.bn1_b = p->bn1_bias; a.noise0 = noise0; a.noise1 = noise1;
+  const AcreTrainLayout L = acre_train_layout(Q, B, a.C, a.par);
+  a.img = ws + L.img; a.y = ws + L.y; a.feat = ws + L.feat; a.a1 = ws + L.a1; a.a2 = ws + L.a2; a.gate = ws + L.gate;
+  a.st0 = ws + L.st0; a.st1 = ws + L.st1; a.part0 = ws + L.part0; a.part1 = ws + L.part1; a.red1 = ws + L.red1;
+  a.dimg = ws + L.dimg;
+  for (int l = 0; l < 3; ++l) { a.pw[l] = ws + L.pw[l]; a.pb[l] = ws + L.pb[l]; }
+  return a;
+}
+
+static int acre_tr_smem_optin(const void* kernel, size_t bytes) {
+  if (bytes > 48 * 1024) KGE_CUDA_OK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+  return KGE_OK;
+}
+
+int64_t kge_acre_train_workspace_bytes(const kge_acre_train_t* p, int64_t Q, int64_t B) {
+  if (!p || B < 1 || acre_train_shape(p, "kge_acre_train_workspace_bytes")) return 0;
+  return acre_train_layout(Q > B ? Q : B, B, p->in_channels, p->way == 1).total * (int64_t)sizeof(float);
+}
+
+int kge_acre_train_fwd(const kge_acre_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                       const float* noise0, const float* noise1, const float* noise2, float* x, void* workspace,
+                       int64_t workspace_bytes, void* stream) {
+  if (int rc = acre_train_check(p, "kge_acre_train_fwd", Q, B)) return rc;
+  if (!e || !r || !x || !workspace) { set_error("kge_acre_train_fwd: null pointer"); return KGE_EINVAL; }
+  if (workspace_bytes < kge_acre_train_workspace_bytes(p, Q, B)) {
+    set_error("kge_acre_train_fwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  const AcreTrain a = acre_train_args(p, e, r, Q, B, noise0, noise1, ws);
+  const AcreTrainLayout L = acre_train_layout(Q, B, a.C, a.par);
+  const ConveTrain cv = acre_tr_view(a, p->bn2_weight, p->bn2_bias, noise2, ws + L.hpre, ws + L.st2, ws + L.red0);
+  const int C = a.C;
+  const long long Fw = acre_feat_width(C);
+  conve_tr_gather_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(cv);
+  KGE_CHECK_LAUNCH("conve_tr_gather_kernel<acre>");
+  conve_tr_bn_stats_kernel<<<1, 256, 0, st>>>(a.part0, Q, B, 1, (float)ACRE_PIX, p->bn0_eps, p->bn0_momentum, a.st0,
+                                              p->bn0_mean, p->bn0_var);
+  KGE_CHECK_LAUNCH("conve_tr_bn_stats_kernel<acre bn0>");
+  if (!a.par) {
+    const size_t smem = (size_t)acre_tr_serial_smem(C).total * sizeof(float);
+    if (int rc = acre_tr_smem_optin((const void*)acre_tr_serial_kernel, smem)) return rc;
+    acre_tr_serial_kernel<<<(unsigned)Q, ACRE_THREADS, smem, st>>>(a);
+    KGE_CHECK_LAUNCH("acre_tr_serial_kernel");
+  } else {
+    const size_t smem = (size_t)acre_tr_gate_smem(C) * sizeof(float);
+    if (int rc = acre_tr_smem_optin((const void*)acre_tr_gate_kernel, smem)) return rc;
+    acre_tr_gate_kernel<<<(unsigned)Q, ACRE_GATE_THREADS, smem, st>>>(a);
+    KGE_CHECK_LAUNCH("acre_tr_gate_kernel");
+    const long long rows = Q * C;
+    if (int rc = launch_gemm<EPI_STORE>(acre_plan_gate(a.gate, p->W_gate_e_weight, p->W_gate_e_bias, rows, a.y,
+                                                       pick_tile(rows, ACRE_PIX)), st, "proj_gemm_kernel<acre train gate>"))
+      return rc;
+  }
+  acre_tr_bn1_part_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("acre_tr_bn1_part_kernel");
+  conve_tr_bn_stats_kernel<<<proj_tiles(C, 256), 256, 0, st>>>(a.part1, Q, B, C, (float)ACRE_PIX, p->bn1_eps,
+                                                              p->bn1_momentum, a.st1, p->bn1_mean, p->bn1_var);
+  KGE_CHECK_LAUNCH("conve_tr_bn_stats_kernel<acre bn1>");
+  acre_tr_feat_kernel<<<proj_tiles(Q * Fw, 256), 256, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("acre_tr_feat_kernel");
+  float* partial = ws + L.partial;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_fc(a.feat, p->fc_weight, Q, Fw, ACRE_K, partial), st,
+                                      "proj_gemm_kernel<acre train fc>")) return rc;
+  conve_tr_fc_combine_kernel<<<proj_tiles(Q * ACRE_K, 256), 256, 0, st>>>(partial, conve_fc_slices(Fw), Q * ACRE_K,
+                                                                          ACRE_K, p->fc_bias, noise2, cv.hpre);
+  KGE_CHECK_LAUNCH("conve_tr_fc_combine_kernel<acre>");
+  conve_tr_bn2_kernel<<<proj_tiles(ACRE_K, 256), 256, 0, st>>>(cv, p->bn2_eps, p->bn2_momentum, p->bn2_mean,
+                                                               p->bn2_var, x);
+  KGE_CHECK_LAUNCH("conve_tr_bn2_kernel<acre>");
+  return KGE_OK;
+}
+
+int kge_acre_train_bwd(const kge_acre_train_t* p, const int64_t* e, const int64_t* r, int64_t Q, int64_t B,
+                       const float* noise0, const float* noise1, const float* noise2, const float* gx, const float* x,
+                       float* const* grads, void* workspace, int64_t workspace_bytes, void* stream) {
+  if (int rc = acre_train_check(p, "kge_acre_train_bwd", Q, B)) return rc;
+  if (!e || !r || !gx || !x || !grads || !workspace) {
+    set_error("kge_acre_train_bwd: null pointer");
+    return KGE_EINVAL;
+  }
+  for (int i = 0; i < KGE_ACRE_TRAIN_GRADS; ++i)
+    if ((grads[i] != nullptr) != acre_train_present(p, i)) {
+      set_error("kge_acre_train_bwd: gradient slot %d must be %s", i, acre_train_present(p, i) ? "set" : "NULL");
+      return KGE_EINVAL;
+    }
+  if (workspace_bytes < kge_acre_train_workspace_bytes(p, Q, B)) {
+    set_error("kge_acre_train_bwd: workspace too small");
+    return KGE_EWORKSPACE;
+  }
+  cudaStream_t st = (cudaStream_t)stream;
+  float* ws = (float*)workspace;
+  const AcreTrain a = acre_train_args(p, e, r, Q, B, noise0, noise1, ws);
+  const AcreTrainLayout L = acre_train_layout(Q, B, a.C, a.par);
+  const ConveTrain cv = acre_tr_view(a, p->bn2_weight, p->bn2_bias, noise2, ws + L.hpre, ws + L.st2, ws + L.red0);
+  const int C = a.C;
+  const long long Fw = acre_feat_width(C);
+  float* dh = ws + L.dh;
+  // grads: ent, rel, bn0.w, bn0.b, conv1.w, conv1.b, conv2.w, conv2.b, conv3.w, conv3.b, W_gate_e.w, W_gate_e.b,
+  //        bn1.w, bn1.b, fc.w, fc.b, bn2.w, bn2.b
+  conve_tr_bn2_bwd_kernel<<<proj_tiles(ACRE_K, 256), 256, 0, st>>>(cv, gx, x, dh, grads[16], grads[17], grads[15]);
+  KGE_CHECK_LAUNCH("conve_tr_bn2_bwd_kernel<acre>");
+  // d fc.weight reads feat before d feat overwrites it (same stream, in order)
+  if (int rc = launch_gemm<EPI_ATOMIC>(conve_plan_grad_fc_w(dh, a.feat, Q, Fw, ACRE_K, grads[14]), st,
+                                       "proj_gemm_kernel<acre grad fc_w>")) return rc;
+  if (int rc = launch_gemm<EPI_STORE>(conve_plan_grad_feat(dh, p->fc_weight, Q, Fw, ACRE_K, a.feat), st,
+                                      "proj_gemm_kernel<acre grad feat>")) return rc;
+  acre_tr_bn1_bwd_part_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("acre_tr_bn1_bwd_part_kernel");
+  conve_tr_reduce_kernel<<<proj_tiles(C, 256), 256, 0, st>>>(a.part1, Q, B, C, a.red1, grads[12], grads[13]);
+  KGE_CHECK_LAUNCH("conve_tr_reduce_kernel<acre bn1>");
+  acre_tr_bn1_bwd_kernel<<<proj_tiles(Q * Fw, 256), 256, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("acre_tr_bn1_bwd_kernel");
+  if (!a.par) {
+    const size_t smem = (size_t)acre_tr_serial_smem(C).total * sizeof(float);
+    if (int rc = acre_tr_smem_optin((const void*)acre_tr_serial_bwd_kernel, smem)) return rc;
+    acre_tr_serial_bwd_kernel<<<(unsigned)Q, ACRE_THREADS, smem, st>>>(a);
+    KGE_CHECK_LAUNCH("acre_tr_serial_bwd_kernel");
+  } else {
+    const long long rows = Q * C;
+    // d W_gate_e.weight reads the gate rows before d gate overwrites them
+    if (int rc = launch_gemm<EPI_ATOMIC>(conve_plan_grad_fc_w(a.feat, a.gate, rows, ACRE_GATE, ACRE_PIX, grads[10]),
+                                         st, "proj_gemm_kernel<acre grad W_gate_e>")) return rc;
+    conve_tr_colsum_kernel<<<proj_tiles(ACRE_PIX, 256), 256, 0, st>>>(a.feat, rows, ACRE_PIX, grads[11]);
+    KGE_CHECK_LAUNCH("conve_tr_colsum_kernel<acre W_gate_e.bias>");
+    if (int rc = launch_gemm<EPI_STORE>(conve_plan_grad_feat(a.feat, p->W_gate_e_weight, rows, ACRE_GATE, ACRE_PIX,
+                                                             a.gate), st, "proj_gemm_kernel<acre grad gate>"))
+      return rc;
+    const size_t smem = (size_t)acre_tr_gate_bwd_smem(C) * sizeof(float);
+    if (int rc = acre_tr_smem_optin((const void*)acre_tr_gate_bwd_kernel, smem)) return rc;
+    acre_tr_gate_bwd_kernel<<<(unsigned)Q, ACRE_GATE_THREADS, smem, st>>>(a);
+    KGE_CHECK_LAUNCH("acre_tr_gate_bwd_kernel");
+  }
+  for (int l = 0; l < 3; ++l) {
+    const int nw = C * acre_tr_cin(l, C, a.par) * 9;
+    conve_tr_colsum_kernel<<<proj_tiles(nw, 256), 256, 0, st>>>(a.pw[l], Q, nw, grads[4 + 2 * l]);
+    KGE_CHECK_LAUNCH("conve_tr_colsum_kernel<acre conv weight>");
+    if (a.has_bias) {
+      conve_tr_colsum_kernel<<<proj_tiles(C, 256), 256, 0, st>>>(a.pb[l], Q, C, grads[5 + 2 * l]);
+      KGE_CHECK_LAUNCH("conve_tr_colsum_kernel<acre conv bias>");
+    }
+  }
+  acre_tr_bn0_part_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(a);
+  KGE_CHECK_LAUNCH("acre_tr_bn0_part_kernel");
+  conve_tr_reduce_kernel<<<1, 256, 0, st>>>(a.part0, Q, B, 1, cv.red0, grads[2], grads[3]);
+  KGE_CHECK_LAUNCH("conve_tr_reduce_kernel<acre bn0>");
+  conve_tr_bn0_bwd_kernel<<<(unsigned)Q, CONVE_TR_THREADS, 0, st>>>(cv, grads[0], grads[1]);
+  KGE_CHECK_LAUNCH("conve_tr_bn0_bwd_kernel<acre>");
   return KGE_OK;
 }
 

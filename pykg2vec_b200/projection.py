@@ -41,8 +41,11 @@ Linear GEMM and bn2 + ReLU.
 
 AcrE (projection.py:621-746) has the same tail and loss; its trunk runs three dilated (atrous) 3x3 convolutions
 on the 20 x 20 image of the stacked entity and relation rows, chained with a residual add (serial way) or side
-by side and mixed per channel by a Linear gate (parallel way).  Training runs the reference's layers;
-evaluation without autograd runs kge_acre_trunk_fwd — one kernel for gather + bn0 + the three convs (+ residual
+by side and mixed per channel by a Linear gate (parallel way).  Training with CUDA tables runs AcreTrunkFunction over
+kge_acre_train_fwd / _bwd (the convolutions blocked in shared memory and registers, W_gate_e on the tiled GEMM, batch
+statistics reduced in a fixed order, dropout as explicit noise tensors) or the Trainer's fused step on the same
+kernels; the reference's layers stay as _trunk_layers for CPU tables, configurations the kernels refuse, BatchNorms
+without a momentum or running statistics, and kge_trunk = False.  Evaluation without autograd runs kge_acre_trunk_fwd — one kernel for gather + bn0 + the three convs (+ residual
 + bn1 + ReLU in the serial way; the gate input in the parallel way, then the gate on the tiled GEMM and bn1 +
 ReLU), then HypER's Linear GEMM and bn2 + ReLU.
 
@@ -862,6 +865,31 @@ class HypER(ProjectionModel):
         return rank
 
 
+class AcreTrunkFunction(torch.autograd.Function):
+    """x = AcrE's trunk in training mode (projection.py:706-734) on kge_acre_train_fwd; backward runs
+    kge_acre_train_bwd.  The Q = G * B rows are G groups of B rows, each with its own batch statistics; the forward
+    updates the model's running statistics in place (num_batches_tracked is the caller's).  noise0 / noise1 / noise2:
+    the dropout noise [Q, 400] / [Q, C] / [Q, 200], or None.  params: AcrE.kge_acre_params().  The backward reuses the
+    forward's feature buffers, so the graph is backpropagated once."""
+
+    @staticmethod
+    def forward(ctx, model, e, r, B, noise0, noise1, noise2, *params):
+        _require_cuda(e, r, *params)
+        params = [t.detach() for t in params]
+        e, r = e.contiguous(), r.contiguous()
+        x, ws = _lib.acre_train_fwd(model, e, r, B, noise0, noise1, noise2, params=params)
+        ctx.model, ctx.B, ctx.noise = model, B, (noise0, noise1, noise2)
+        ctx.save_for_backward(e, r, x, ws, *params)
+        return x
+
+    @staticmethod
+    def backward(ctx, gx):
+        e, r, x, ws, *params = ctx.saved_tensors
+        grads = [torch.zeros_like(t) for t in params]
+        _lib.acre_train_bwd(ctx.model, e, r, ctx.B, gx.contiguous(), x, grads, ws, *ctx.noise, params=params)
+        return (None,) * 7 + tuple(g if need else None for g, need in zip(grads, ctx.needs_input_grad[7:]))
+
+
 class AcrE(ProjectionModel):
     """pykg2vec/models/projection.py:621-746 — same kwargs, sub-module names and state_dict keys and order (bias /
     ent_embeddings / rel_embeddings / bn0 / bn1 / bn2 / fc / conv1 / conv2 / conv3, then W_gate_e in the parallel
@@ -871,8 +899,12 @@ class AcrE(ProjectionModel):
     10 x 20, so hidden_size must be 200 for the reference's forward to mean anything; the class constructs for
     any size, as upstream, and the evaluation kernel refuses the others (KgeNotSupported).
 
-    Training runs the reference's layers (the three convolutions through _Fp32Conv2d with their dilation and
-    padding, TF32 off); evaluation without autograd runs kge_acre_trunk_fwd."""
+    In training mode with the tables on a CUDA device the trunk is AcreTrunkFunction (kge_acre_train_*); the
+    reference's torch layers (the three convolutions through _Fp32Conv2d with their dilation and padding, TF32 off)
+    stay as _trunk_layers: the yardstick of the tests, the path for CPU tables, for configurations the kernels refuse
+    (hidden_size != 200, where the reference's own view error surfaces, or more channels than they take), for
+    BatchNorms with momentum None or without running statistics and, with the attribute / kwarg kge_trunk = False,
+    for everything.  Evaluation without autograd runs kge_acre_trunk_fwd."""
 
     def __init__(self, **kwargs):
         super(AcrE, self).__init__(self.__class__.__name__.lower())
@@ -906,12 +938,80 @@ class AcrE(ProjectionModel):
         nn.init.xavier_uniform_(self.rel_embeddings.weight.data)
         self.parameter_list = [self.ent_embeddings, self.rel_embeddings]
         self.loss = Criterion.multi_class_bce
+        self.kge_trunk = bool(kwargs.get("kge_trunk", True))
 
     def embed(self, h, r, t):
         return self.ent_embeddings(h), self.rel_embeddings(r), self.ent_embeddings(t)
 
     def embed2(self, e, r):
         return self.ent_embeddings(e), self.rel_embeddings(r)
+
+    def _kernel_trunk(self):
+        """the kernels are selected and the tables live on a CUDA device (the kernels read device memory only)"""
+        return self.kge_trunk and self.ent_embeddings.weight.is_cuda
+
+    def kge_train_supported(self):
+        """kge_acre_train_* runs this model's training trunk: kernels selected, a configuration they take
+        (hidden_size 200; serial in_channels <= 46, parallel <= 1024) and BatchNorms with running statistics and a
+        momentum"""
+        bns = (self.bn0, self.bn1, self.bn2)
+        return self._kernel_trunk() and all(bn.track_running_stats and bn.momentum is not None for bn in bns) and \
+            self._kge_train_config_ok()
+
+    def _kge_train_config_ok(self):
+        """kge_acre_train_workspace_bytes accepts this configuration: asked once per configuration, not per step"""
+        key = (self.way, int(self.in_channels), int(self.ent_embeddings.weight.shape[1]),
+               int(self.rel_embeddings.weight.shape[0]), int(self.first_atrous), int(self.second_atrous),
+               int(self.third_atrous))
+        if getattr(self, "_kge_train_ok", (None,))[0] != key:
+            self._kge_train_ok = (key, _lib.acre_train_workspace_bytes(self, 2, 2) > 0)
+        return self._kge_train_ok[1]
+
+    def kge_acre_params(self):
+        """the trunk tensors this model has, in kge_acre_train_bwd's slot order (parameters() without the bias row):
+        ent, rel, bn0.*, conv1.*, conv2.*, conv3.* (biases with acre_bias only), W_gate_e.* (parallel way only),
+        bn1.*, fc.*, bn2.*"""
+        out = [self.ent_embeddings.weight, self.rel_embeddings.weight, self.bn0.weight, self.bn0.bias]
+        for conv in (self.conv1, self.conv2, self.conv3):
+            out += [conv.weight] + ([conv.bias] if conv.bias is not None else [])
+        if self.way != "serial":
+            out += [self.W_gate_e.weight, self.W_gate_e.bias]
+        return out + [self.bn1.weight, self.bn1.bias, self.fc.weight, self.fc.bias, self.bn2.weight, self.bn2.bias]
+
+    def dropout_noise(self, rows):
+        """(noise0 [rows, 400], noise1 [rows, C], noise2 [rows, 200]) of inp_drop (on the [rows, 1, 20, 20] image),
+        feature_map_drop (Dropout2d: one value per channel) and hidden_drop in training mode, drawn in that order as
+        ATen draws bernoulli noise: each None when its p is 0 or in eval mode, zeros when p >= 1"""
+        w = self.ent_embeddings.weight
+        out = []
+        for drop, width in ((self.inp_drop, 400), (self.feature_map_drop, int(self.in_channels)),
+                            (self.hidden_drop, int(self.hidden_size))):
+            p = float(drop.p)
+            if p == 0.0 or not self.training:
+                out.append(None)
+            elif p >= 1.0:
+                out.append(torch.zeros((rows, width), dtype=torch.float32, device=w.device))
+            else:
+                out.append(torch.empty((rows, width), dtype=torch.float32, device=w.device).bernoulli_(1 - p)
+                           .div_(1 - p))
+        return tuple(out)
+
+    def note_batch_stats(self, forwards=1):
+        """num_batches_tracked += forwards on the three BatchNorms (kge_acre_train_fwd updates the rest)"""
+        for bn in (self.bn0, self.bn1, self.bn2):
+            bn.num_batches_tracked.add_(forwards)
+
+    def _train_trunk(self, e, r):
+        """the training-mode trunk: AcreTrunkFunction where the kernels take it, else the torch layers"""
+        B = e.shape[0]
+        if B == 0 or not self.kge_train_supported():
+            return self._trunk_layers(e, r)
+        if B == 1:   # nn.BatchNorm1d's refusal (bn2), before anything runs
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % (torch.Size([1, int(self.hidden_size)]),))
+        x = AcreTrunkFunction.apply(self, e, r, B, *self.dropout_noise(B), *self.kge_acre_params())
+        self.note_batch_stats()
+        return x
 
     # ---- trunk: AcrE.forward before the x . E^T product (projection.py:708-734) ----
     def _trunk_layers(self, e, r):
@@ -948,7 +1048,7 @@ class AcrE(ProjectionModel):
         _require_cuda(e, r, self.ent_embeddings.weight)
         if not self.training and not torch.is_grad_enabled():
             return _lib.acre_trunk_fwd(self, e.contiguous(), r.contiguous())
-        return self._trunk_layers(e, r)
+        return self._train_trunk(e, r) if self.training else self._trunk_layers(e, r)
 
     def proj_tail_tables(self):
         """(entity table [N,k], bias row [N]) of the tail product."""

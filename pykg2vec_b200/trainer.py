@@ -26,6 +26,8 @@ Two execution modes for the same step semantics:
                              kge_hyper_train_bwd -> kge_optim_apply_dense over all 13 parameter tensors
       InteractE            : kge_interacte_train_fwd (both directions, per-direction batch statistics) -> tail + BCE
                              -> kge_interacte_train_bwd -> kge_optim_apply_dense over all 12 parameter tensors
+      AcrE                 : kge_acre_train_fwd (both directions, per-direction batch statistics) -> tail + BCE ->
+                             kge_acre_train_bwd -> kge_optim_apply_dense over every parameter tensor
   * data-parallel (torch.distributed world > 1, tables replicated; SURVEY.md 8e row 3): config.dp_mode
       "grads": every rank scores ITS batch shard forward + backward into the dense gradient buffers,
                ONE all-reduce per table sums (hinge) / averages (mean-type losses) them over NVLink, then
@@ -69,6 +71,7 @@ class Trainer:
         self._conve = False
         self._hyper = False
         self._interacte = False
+        self._acre = False
 
     def build_model(self):
         """trainer.py:103-144 (optimizer selection; unknown names raise NotImplementedError)."""
@@ -127,6 +130,13 @@ class Trainer:
         self._interacte = name in ("sgd", "adagrad", "adam") and getattr(self.config, "fused_step", True) and \
             self.model.model_name.lower() == "interacte" and self.model.kge_train_supported()
         if self._interacte:
+            params = list(self.model.parameters())
+            self._grad_scratch = [torch.zeros_like(t) for t in params]
+            self._state = [torch.zeros_like(t) for t in params] if name in ("adagrad", "adam") else None
+            self._state2 = [torch.zeros_like(t) for t in params] if name == "adam" else None
+        self._acre = name in ("sgd", "adagrad", "adam") and getattr(self.config, "fused_step", True) and \
+            self.model.model_name.lower() == "acre" and self.model.kge_train_supported()
+        if self._acre:
             params = list(self.model.parameters())
             self._grad_scratch = [torch.zeros_like(t) for t in params]
             self._state = [torch.zeros_like(t) for t in params] if name in ("adagrad", "adam") else None
@@ -497,6 +507,50 @@ class Trainer:
                                    self._state2[k] if self._state2 else None, step=self._step)
         return loss
 
+    def _fused_acre(self, ids):
+        """AcrE: train_step_projection (trainer.py:159-174) + backward + optimizer.step() without an autograd graph.
+        Both directions run as ONE trunk launch sequence over 2B rows (AcrE indexes rel with r in both directions), each
+        direction with its own batch statistics and the running statistics updated tail first; then the shared tail,
+        the BCE loss and its gradient per direction, the tail's backward, the trunk's, and one dense optimizer sweep
+        over every parameter tensor (all get a gradient every step, as under loss.backward())."""
+        h, r, t, hr_t, tr_h = ids
+        m = self.model
+        B = r.numel()
+        if B == 1:   # nn.BatchNorm1d's refusal (bn2), before anything runs
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % (torch.Size([1, int(m.hidden_size)]),))
+        plist = list(m.parameters())   # bias, ent, rel, bn0.*, bn1.*, bn2.*, fc.*, conv1..3.*, [W_gate_e.*]
+        at = {id(w): i for i, w in enumerate(plist)}
+        order = [at[id(w)] for w in m.kge_acre_params()]
+        params = [w.detach() for w in plist]
+        trunk = [params[i] for i in order]
+        ent, bias = m.ent_embeddings.weight.detach(), m.bias.detach()
+        e2, r2 = torch.cat([h, t]), torch.cat([r, r])   # rows [0, B): tail direction, [B, 2B): head
+        nt, nh = m.dropout_noise(B), m.dropout_noise(B)   # the reference's draw order: tail forward, then head
+        noise = [None if a is None else torch.cat([a, b]) for a, b in zip(nt, nh)]
+        x, ws = _lib.acre_train_fwd(m, e2, r2, B, *noise, params=trunk)
+        m.note_batch_stats(2)
+        preds = _lib.proj_tail_fwd(x, ent, bias)
+        scale, shift = 1.0, 0.0
+        if hasattr(self.config, "label_smoothing"):
+            scale, shift = 1.0 - self.config.label_smoothing, 1.0 / self.config.tot_entity
+        grads = self._grad_scratch
+        gent, gb = grads[at[id(m.ent_embeddings.weight)]], grads[at[id(m.bias)]]
+        gx = torch.zeros_like(x)
+        loss = None
+        for lo, lab in ((0, hr_t), (B, tr_h)):
+            part, gp = _lib.proj_bce(preds[lo:lo + B], lab.to(torch.float32).contiguous(), scale, shift)
+            _lib.proj_tail_bwd(gp, preds[lo:lo + B], x[lo:lo + B], ent, gx[lo:lo + B], gent, gb)
+            loss = part if loss is None else loss + part
+        del preds, gp
+        _lib.acre_train_bwd(m, e2, r2, B, gx, x, [grads[i] for i in order], ws, *noise, params=trunk)
+        self._step += 1
+        lr = float(self.config.learning_rate)
+        for k, w in enumerate(params):
+            _lib.optim_apply_dense(w, grads[k], self._opt_code(), lr, self._state[k] if self._state else None,
+                                   self._state2[k] if self._state2 else None, step=self._step)
+        return loss
+
     # ---- one batch, host ids in, host loss out (trainer.py:269-300) -----------------------------
     def _to_device(self, arrays):
         """Pack the batch's id arrays into one pinned staging buffer and issue ONE H2D copy
@@ -605,6 +659,9 @@ class Trainer:
         if self._interacte:
             with torch.no_grad():
                 return self._fused_interacte(ids)
+        if self._acre:
+            with torch.no_grad():
+                return self._fused_acre(ids)
         if self._fused:
             with torch.no_grad():
                 if strategy == TrainingStrategy.PAIRWISE_BASED:
@@ -655,7 +712,7 @@ class Trainer:
         else:
             ids, nbytes = self._to_device(list(data))
         self.last_h2d_bytes = nbytes
-        if self._fused or self._proje or self._tucker or self._conve or self._hyper or self._interacte:
+        if self._fused or self._proje or self._tucker or self._conve or self._hyper or self._interacte or self._acre:
             loss = self.train_batch_device(ids)
             if not sync:
                 return loss                # device tensor; float(loss) syncs when the caller wants the value
