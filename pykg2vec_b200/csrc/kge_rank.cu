@@ -17,6 +17,7 @@
 //     register-tiled pair evaluation, FMA-pipe bound.
 #include "kge_models.cuh"
 #include "kge_rank.cuh"
+#include "kge_rank_resolve.cuh"
 
 namespace kge {
 
@@ -76,67 +77,13 @@ threshold_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t* _
   if (valid && lane == 0) thr[g] = s;
 }
 
-// Exact re-evaluation of listed (query, candidate) pairs with the canonical fp32 group function — the
-// arithmetic of kge_score_fwd and of the sweeps.  One 8-lane group per item:
-//   items [0, total)            : with a band list (ctrl != nullptr), the pairs whose tensor-core accumulator
-//                                 fell inside the query's band (kge_rank_tc.cu): tc_counts[q] += 1 when the
-//                                 candidate really outranks the target.  total = 0 when the list overflowed.
-//   items [total, total + nnz)  : the filter entries: the filtered column -= 1 when the entry outranks the
-//                                 target.  Entries equal to the target or outside the row shard are skipped.
-// With a band list the fp32 tiled sweep enqueued behind this kernel then commits the direction (counts +=
-// tc_counts) or — list overflow: ctrl[0] > cap or ctrl[1] — ranks it itself (sweep_tiled_body's entry,
-// kge_rank_tiled.cu); on overflow this kernel still applies the filter corrections.
+// the filter pass of the gather and fp32 paths: exact re-evaluation of the filter entries (kge_rank_resolve.cuh)
 template <int MODEL, int VEC, int GROUPING>
-__global__ void __launch_bounds__(kThreads)
-resolve_pairs_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t* __restrict__ qr,
-                     const int64_t* __restrict__ qt, const float* __restrict__ thr,
-                     const unsigned long long* __restrict__ list, unsigned* __restrict__ ctrl, unsigned cap,
-                     int32_t* __restrict__ tc_counts, const RankFilter F, int64_t Q, int64_t row_lo, int64_t row_hi,
-                     int32_t* __restrict__ counts, int col, int scratch_floats) {
+__global__ void __launch_bounds__(kResolveThreads)
+resolve_pairs_kernel(const __grid_constant__ ModelParams P, const __grid_constant__ ResolveArgs A) {
   extern __shared__ float4 smem_f4[];
-  float* scratch = reinterpret_cast<float*>(smem_f4) + (size_t)(threadIdx.x >> 3) * scratch_floats;
-  const int lane = threadIdx.x & 7;
-  const unsigned listed = ctrl ? *reinterpret_cast<volatile unsigned*>(&ctrl[0]) : 0u;
-  const bool overflow = listed > cap || (ctrl && *reinterpret_cast<volatile unsigned*>(&ctrl[1]) != 0u);
-  const int64_t total = overflow ? 0 : (int64_t)listed;
-  // the true entry count lives in device memory (ptr[Q]); the host may pass a capacity
-  // (upper bound) as nnz so that the launch shape can stay fixed inside a CUDA graph
-  const int64_t nnz_true = (F.ptr && F.idx && F.nnz > 0) ? min(F.nnz, __ldg(F.ptr + Q)) : 0;
-  const int64_t items = total + nnz_true;
-  for (int64_t k = (int64_t)blockIdx.x * kGroupsPerCta + (threadIdx.x >> 3); k < items;
-       k += (int64_t)gridDim.x * kGroupsPerCta) {
-    int64_t q, e;
-    bool skip = false;
-    const bool band = k < total;
-    if (band) {
-      const unsigned long long pr = list[k];
-      if (pr == ~0ull) continue;   // unused slot of a warp's reserved block (kge_rank_tc.cu); group-uniform
-      q = (int64_t)(pr >> 32);
-      e = (int64_t)(pr & 0xffffffffull);
-    } else {
-      const int64_t kk = k - total;
-      int64_t lo = 0, hi = Q;  // largest q with ptr[q] <= kk
-      while (hi - lo > 1) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (__ldg(F.ptr + mid) <= kk) lo = mid; else hi = mid;
-      }
-      q = lo;
-      const int64_t ge = __ldg(F.idx + kk);
-      skip = (ge == __ldg(F.tgt + q)) || ge < row_lo || ge >= row_hi;
-      e = skip ? 0 : ge - row_lo;
-    }
-    TripleRows R;
-    if (GROUPING == KGE_GROUP_TAIL)
-      resolve_rows<MODEL>(R, P, P.qtab, P.tab, P.qtab, __ldg(qh + q), __ldg(qr + q), e);
-    else
-      resolve_rows<MODEL>(R, P, P.tab, P.qtab, P.qtab, e, __ldg(qr + q), __ldg(qt + q));
-    prefetch_triple_rows(R, P.d, P.dr, lane);
-    const float s = score_group<MODEL, VEC, GROUPING>(R, P, lane, scratch);
-    if (lane == 0 && !skip && s < __ldg(thr + q)) {
-      if (band) atomicAdd(tc_counts + q, 1);
-      else atomicSub(counts + q * 4 + col + 1, 1);
-    }
-  }
+  float* scratch = reinterpret_cast<float*>(smem_f4) + (size_t)(threadIdx.x >> 3) * A.scratch_floats;
+  resolve_items<MODEL, VEC, GROUPING>(P, A, 0, scratch);
 }
 
 SweepProfile* sweep_profile(int dir) {
@@ -173,15 +120,14 @@ RankLayout rank_layout(const kge_model_t* m, int64_t Q) {
       }
       for (int k = 0; k < 2; ++k) L.b[k] = take((size_t)m->num_ent * Kp * 2);
       L.cn = take((size_t)m->num_ent * sizeof(float));
+      if (m->model == KGE_TRANSE) L.cinv = take((size_t)m->num_ent * sizeof(float));
     }
   }
   L.total = o;
   return L;
 }
 
-// launch parameters of the group-function kernels of this file
-struct GroupArgs { ModelParams P; int vec, sf; size_t smem; };
-static GroupArgs group_args(const RankCall& C) {
+GroupArgs group_args(const RankCall& C) {
   GroupArgs G;
   G.P = make_params(C.m, C.mq);
   G.vec = model_vec(C.m);
@@ -221,9 +167,23 @@ static int gather_sweep(const RankCall& C, int dir, cudaStream_t st) {
   return KGE_OK;
 }
 
+ResolveArgs resolve_args(const RankCall& C, int dir) {
+  ResolveArgs A;
+  A.qh = C.qh; A.qr = C.qr; A.qt = C.qt; A.thr = C.thr(dir);
+  A.list = C.use_tc ? C.at<unsigned long long>(C.L.list[dir]) : nullptr;
+  A.ctrl = C.use_tc ? C.at<unsigned>(C.L.ctrl[dir]) : nullptr;
+  A.cap = tc_list_capacity(C.Q);
+  A.tc_counts = C.use_tc ? C.at<int32_t>(C.L.tc_counts[dir]) : nullptr;
+  A.F = C.filt[dir];
+  A.Q = C.Q; A.row_lo = C.row_lo; A.row_hi = C.row_hi;
+  A.counts = C.counts; A.col = 2 * dir;
+  A.scratch_floats = (int)group_scratch_floats(C.m);
+  return A;
+}
+
 int resolve_pairs(const RankCall& C, int dir, cudaStream_t st) {
   const RankFilter& F = C.filt[dir];
-  if (!C.use_tc && !(F.ptr && F.idx && F.nnz > 0)) return KGE_OK;
+  if (!(F.ptr && F.idx && F.nnz > 0)) return KGE_OK;
   const GroupArgs G = group_args(C);
   decltype(&resolve_pairs_kernel<KGE_TRANSE, 4, KGE_GROUP_TAIL>) kernel;
 #define PICK(M, V) kernel = dir == 0 ? resolve_pairs_kernel<M, V, KGE_GROUP_TAIL> : resolve_pairs_kernel<M, V, KGE_GROUP_HEAD>
@@ -231,24 +191,22 @@ int resolve_pairs(const RankCall& C, int dir, cudaStream_t st) {
 #undef PICK
   const int rc = smem_optin(kernel, G.smem);
   if (rc) return rc;
-  // the band list's length is only known on the device: grid-stride over two CTAs per SM;
-  // filters alone: one group per entry
-  const unsigned grid = C.use_tc ? (unsigned)(2 * sm_count()) : (unsigned)((F.nnz + kGroupsPerCta - 1) / kGroupsPerCta);
-  kernel<<<grid, kThreads, G.smem, st>>>(
-      G.P, C.qh, C.qr, C.qt, C.thr(dir), C.use_tc ? C.at<unsigned long long>(C.L.list[dir]) : nullptr,
-      C.use_tc ? C.at<unsigned>(C.L.ctrl[dir]) : nullptr, tc_list_capacity(C.Q),
-      C.use_tc ? C.at<int32_t>(C.L.tc_counts[dir]) : nullptr, F, C.Q, C.row_lo, C.row_hi, C.counts, 2 * dir, G.sf);
+  // one group per entry
+  const unsigned grid = (unsigned)((F.nnz + kResolveGroups - 1) / kResolveGroups);
+  kernel<<<grid, kResolveThreads, G.smem, st>>>(G.P, resolve_args(C, dir));
   KGE_CHECK_LAUNCH("resolve_pairs_kernel");
   return KGE_OK;
 }
 
 // Fork/join helper: the head-direction chain of a rank call runs on a side stream so that its
 // short preparation / filter kernels overlap the other direction's sweep (and fill the idle
-// SMs of its last wave).  Streams and events are created lazily, once per host thread and device;
-// event record / wait are capture-safe, so the pattern also works inside a CUDA graph capture.
+// SMs of its last wave); with the tensor-core sweep the two query preparations run on the two side
+// streams beside the candidate preparation.  Streams and events are created lazily, once per host
+// thread and device; event record / wait are capture-safe, so the pattern also works inside a CUDA
+// graph capture.
 struct SideStream {
-  cudaStream_t stream = nullptr;
-  cudaEvent_t fork = nullptr, join = nullptr, mid = nullptr, fork2 = nullptr;
+  cudaStream_t stream = nullptr, stream2 = nullptr;
+  cudaEvent_t fork = nullptr, join = nullptr, mid = nullptr, mid2 = nullptr, fork2 = nullptr;
   int device = -1;
 };
 static int side_stream(SideStream** out) {
@@ -258,9 +216,11 @@ static int side_stream(SideStream** out) {
   SideStream& s = ss[dev & 15];
   if (!s.stream) {
     KGE_CUDA_OK(cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking));
+    KGE_CUDA_OK(cudaStreamCreateWithFlags(&s.stream2, cudaStreamNonBlocking));
     KGE_CUDA_OK(cudaEventCreateWithFlags(&s.fork, cudaEventDisableTiming));
     KGE_CUDA_OK(cudaEventCreateWithFlags(&s.join, cudaEventDisableTiming));
     KGE_CUDA_OK(cudaEventCreateWithFlags(&s.mid, cudaEventDisableTiming));
+    KGE_CUDA_OK(cudaEventCreateWithFlags(&s.mid2, cudaEventDisableTiming));
     KGE_CUDA_OK(cudaEventCreateWithFlags(&s.fork2, cudaEventDisableTiming));
     s.device = dev;
   }
@@ -321,10 +281,6 @@ extern "C" int kge_rank_1vsall(const kge_model_t* m, const kge_model_t* mq, int6
   C.use_tiled = !(flags & KGE_RANK_FORCE_GATHER) && tiled_supported(m);
   C.use_tc = C.use_tiled && !(flags & KGE_RANK_NO_TC) && tc_supported(m, C.nc);
   const cudaStream_t main_st = (cudaStream_t)stream;
-  if (C.use_tiled) {
-    rc = prepare_candidates(C, main_st);
-    if (rc) return rc;
-  }
   for (int d = 0; d < 2; ++d) {
     SweepProfile* sp = sweep_profile(d);
     sp->armed = (flags & KGE_RANK_PROFILE) != 0;
@@ -339,27 +295,40 @@ extern "C" int kge_rank_1vsall(const kge_model_t* m, const kge_model_t* mq, int6
   // (CP / SimplE refill one shared candidate scratch per direction: their directions stay serial)
   const bool dirs_independent = m->model != KGE_CP && !is_simple(m->model);
   const bool two_streams = run[0] && run[1] && C.use_tiled && dirs_independent && !(flags & KGE_RANK_SINGLE_STREAM);
-  // Both directions on the tensor cores: their query preparations run side by side, ONE launch sweeps both
-  // (grid.z = 2: same candidate operands; the launch / pipeline-ramp / drain overhead — a third of a 25 us
-  // sweep at the FB15k-237 shape — is paid once and the tile units of both directions balance over the SMs),
-  // then the two exact-resolution chains run side by side again.
+  // Both directions on the tensor cores: the two query preparations run on the two side streams from the start,
+  // beside the candidate preparation (they read none of its outputs), ONE launch sweeps both directions (grid.z = 2:
+  // same candidate operands; the launch / pipeline-ramp / drain overhead — a third of a 25 us sweep at the
+  // FB15k-237 shape — is paid once and the tile units of both directions balance over the SMs), then the two
+  // resolve-and-commit launches run side by side.
   const bool tc_both = C.use_tc && two_streams;
   SideStream* side = nullptr;
+  auto fork = [&]() {
+    KGE_CUDA_OK(cudaEventRecord(side->fork, main_st));
+    KGE_CUDA_OK(cudaStreamWaitEvent(side->stream, side->fork, 0));
+    if (tc_both) KGE_CUDA_OK(cudaStreamWaitEvent(side->stream2, side->fork, 0));
+    return KGE_OK;
+  };
   if (two_streams) {
     rc = side_stream(&side);
     if (rc) return rc;
-    KGE_CUDA_OK(cudaEventRecord(side->fork, main_st));          // after candidate preparation
-    KGE_CUDA_OK(cudaStreamWaitEvent(side->stream, side->fork, 0));
   }
+  if (tc_both && (rc = fork())) return rc;
+  if (C.use_tiled) {
+    rc = prepare_candidates(C, main_st);
+    if (rc) return rc;
+  }
+  if (two_streams && !tc_both && (rc = fork())) return rc;   // the fp32 sweeps read the prepared candidates
   auto stream_of = [&](int dir) { return (two_streams && dir == 1) ? side->stream : main_st; };
   auto resolve_and_sweep = [&](int dir) {
+    if (C.use_tc) return tc_resolve_commit(C, dir, stream_of(dir));
     const int r = resolve_pairs(C, dir, stream_of(dir));
     if (r) return r;
     return C.use_tiled ? tiled_sweep(C, dir, stream_of(dir)) : gather_sweep(C, dir, stream_of(dir));
   };
   for (int dir = 0; dir < 2; ++dir) {
     if (!run[dir]) continue;
-    rc = C.use_tiled ? prepare_queries(C, dir, stream_of(dir)) : gather_thresholds(C, dir, stream_of(dir));
+    const cudaStream_t prep_st = tc_both ? (dir == 0 ? side->stream : side->stream2) : stream_of(dir);
+    rc = C.use_tiled ? prepare_queries(C, dir, prep_st) : gather_thresholds(C, dir, prep_st);
     if (rc) return rc;
     if (tc_both) continue;
     if (C.use_tc) {
@@ -371,7 +340,9 @@ extern "C" int kge_rank_1vsall(const kge_model_t* m, const kge_model_t* mq, int6
   }
   if (tc_both) {
     KGE_CUDA_OK(cudaEventRecord(side->mid, side->stream));
+    KGE_CUDA_OK(cudaEventRecord(side->mid2, side->stream2));
     KGE_CUDA_OK(cudaStreamWaitEvent(main_st, side->mid, 0));
+    KGE_CUDA_OK(cudaStreamWaitEvent(main_st, side->mid2, 0));
     rc = tc_sweep(C, 0, 2, nullptr, main_st);
     if (rc) return rc;
     KGE_CUDA_OK(cudaEventRecord(side->fork2, main_st));
@@ -417,8 +388,7 @@ extern "C" int kge_rank_tc_probe(const kge_model_t* m, const kge_model_t* mq, in
     KGE_CUDA_OK(cudaMemcpyAsync(tau, C.ws + C.L.tau[direction], (size_t)Q * 4 * sizeof(float), cudaMemcpyDeviceToDevice, st));
     KGE_CUDA_OK(cudaMemcpyAsync(tau + (size_t)Q * 4, C.ws + C.L.cn, (size_t)C.nc * sizeof(float), cudaMemcpyDeviceToDevice, st));
   }
-  if ((rc = resolve_pairs(C, direction, st))) return rc;
-  return tiled_sweep(C, direction, st);
+  return tc_resolve_commit(C, direction, st);
 }
 
 extern "C" int kge_rank_last_sweep_directions(void) {

@@ -40,14 +40,16 @@ struct RankLayout {
   size_t thr[2];               // [Q] thresholds: the target's own score
   size_t qvec[2];              // [Q][KQ][dp] query vectors of the tiled sweep
   size_t qscale[2];            // [Q] TransM scale theta[r]
-  size_t cand;                 // [KC][num_ent][dp] candidate scratch (normalised / padded / realigned rows)
+  size_t cand;                 // [KC][num_ent][dp] candidate scratch (normalised / padded / realigned rows); unused
+                               // by TransE on the tensor-core path when the fallback can read the table itself
   size_t a[2][2];              // [dir][0: high, 1: low] bf16 query operands [Q][Kp]
   size_t tau[2];               // [Q][4] band coefficients (centre, a, b, e) of tc_query_finish
   size_t tc_counts[2];         // [Q] certain counts of level 1 (+ the resolved pairs of level 2)
-  size_t ctrl[2];              // [4] pair-list length, overflow (+ 2 unused words)
+  size_t ctrl[2];              // [4] pair-list length, overflow, resolve-and-commit done counter (+ 1 unused)
   size_t list[2];              // [tc_list_capacity(Q)] (q << 32 | local candidate row)
   size_t b[2];                 // [0: high, 1: low] bf16 candidate operands [num_ent][Kp]
   size_t cn;                   // [num_ent] candidate norm bounds
+  size_t cinv;                 // [num_ent] TransE: the canonical inverse norm of every candidate row
   size_t total;
 };
 RankLayout rank_layout(const kge_model_t* m, int64_t Q);
@@ -79,19 +81,22 @@ struct RankCall {
 //                        query operands and band coefficients; CP's per-direction candidate operands first
 //   tc_sweep             level 1 of one direction, or of both (ndirs == 2, dir == 0) in one grid.z = 2 launch;
 //                        dots: optional [Q][nc] raw accumulators of direction `dir` (tests)
-//   resolve_pairs        exact fp32 re-evaluation of listed pairs: the filter corrections, and with use_tc the
-//                        ambiguous pairs of level 1 into tc_counts
-//   tiled_sweep          the fp32 sweep; with use_tc its entry commits tc_counts to counts instead, unless the
-//                        pair list overflowed
+//   tc_resolve_commit    use_tc, one launch: exact fp32 re-evaluation of the ambiguous pairs of level 1 and of the
+//                        filter entries, then counts += tc_counts; or, when the pair list overflowed, the fp32
+//                        tiled sweep of the direction and the filter corrections
+//   resolve_pairs        without use_tc: exact fp32 re-evaluation of the filter entries (the filter corrections)
+//   tiled_sweep          without use_tc: the fp32 sweep
 int prepare_candidates(const RankCall& C, cudaStream_t st);
 int prepare_queries(const RankCall& C, int dir, cudaStream_t st);
 int tc_sweep(const RankCall& C, int dir, int ndirs, float* dots, cudaStream_t st);
+int tc_resolve_commit(const RankCall& C, int dir, cudaStream_t st);
 int resolve_pairs(const RankCall& C, int dir, cudaStream_t st);
 int tiled_sweep(const RankCall& C, int dir, cudaStream_t st);
 
 // Used by the preparation stages of kge_rank_tiled.cu.  src[k]: the fp32 candidate tables (row pitch m->dim);
-// scratch: optional fp32 copy [KC][nc][dp] for the fp32 fallback sweep, written by the same kernel.
-int tc_prepare_candidates(const RankCall& C, const float* const src[2], float* scratch, cudaStream_t st);
+// scratch: optional fp32 copy [KC][nc][dp] for the fp32 fallback sweep, written by the same kernel; cinv
+// (TransE): optional [nc] inverse row norms, with which the fallback normalises the raw rows it stages.
+int tc_prepare_candidates(const RankCall& C, const float* const src[2], float* scratch, float* cinv, cudaStream_t st);
 struct TcQueryArgs;
 TcQueryArgs tc_query_args(const RankCall& C, int dir);
 

@@ -23,8 +23,8 @@
 //     the fp32 sweeps / the CPU oracle) and compared exactly.
 //
 // The final counts therefore equal the fp32 specification's for every input.  If the list
-// overflows (degenerate tables: thousands of exact ties per query) the fp32 tiled sweep of
-// kge_rank_tiled.cu runs instead, decided on the device (no host sync).
+// overflows (degenerate tables: thousands of exact ties per query) the resolve launch runs the fp32
+// tiled sweep of kge_rank_tiled.cu instead, decided on the device (no host sync).
 //
 // Replaces: Evaluator.test_tail_rank / test_head_rank forward over all N entities + topk
 // (pykg2vec/utils/evaluator.py:249-273,309-334) for models pairwise.py:56-93 (TransE, -l1 False),
@@ -53,7 +53,7 @@ constexpr int kTcResidentMaxK = 256;                   // query block stays in s
 struct TcDirView {
   const float* tau;        // [Q][4]: centre, a, b, e (tc_query_finish)
   int32_t* tc_counts;      // [Q]
-  unsigned* ctrl;          // [0] list length, [1] overflow ([2], [3] unused)
+  unsigned* ctrl;          // [0] list length, [1] overflow ([2] tc_resolve_commit_kernel's done counter)
   unsigned long long* list;
   float* dbg;              // optional [Q][nc] raw accumulators (tests)
 };
@@ -389,16 +389,16 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
 
 // ---- operand preparation --------------------------------------------------------------------------
 // One 8-lane group per candidate row, ONE pass over the fp32 table(s) for everything the row needs:
-// (NORMALISE: TransE) the canonical row normalisation of the fp32 sweep's scratch copy — same arithmetic
-// as prep_cand_kernel, written to s0 when the caller keeps that scratch for the fp32 fallback —, the bf16
-// split of the KC arrays concatenated along k, the three norm columns (squared-distance models) and the
-// row's norm bound n_c.  Rows are read with the widest vector the table alignment allows; columns
-// d .. dp-1 are zero.
+// (NORMALISE: TransE) the canonical row normalisation of the fp32 sweep — same arithmetic as prep_cand_kernel;
+// the fp32 fallback gets either its inverse norm (cinv, when it stages the raw table) or the normalised rows
+// (s0, a scratch copy) —, the bf16 split of the KC arrays concatenated along k, the three norm columns
+// (squared-distance models) and the row's norm bound n_c.  Rows are read with the widest vector the table
+// alignment allows; columns d .. dp-1 are zero.
 template <int VEC, bool NORMALISE>
 __global__ void __launch_bounds__(256)
 tc_prep_cand_kernel(const float* __restrict__ c0, const float* __restrict__ c1, int64_t pitch, int64_t nc, int d,
                     int dp, int KC, int Kp, int aug, __nv_bfloat16* __restrict__ B0, __nv_bfloat16* __restrict__ B1,
-                    float* __restrict__ cn, float* __restrict__ s0, float* __restrict__ s1) {
+                    float* __restrict__ cn, float* __restrict__ s0, float* __restrict__ s1, float* __restrict__ cinv) {
   const int lane = threadIdx.x & 7;
   const int64_t e = (int64_t)blockIdx.x * 32 + (threadIdx.x >> 3);
   if (e >= nc) return;
@@ -419,6 +419,7 @@ tc_prep_cand_kernel(const float* __restrict__ c0, const float* __restrict__ c1, 
         for (int j = 0; j < 4; ++j) s = ffma(f4_get(x, j), f4_get(x, j), s);
       }
       inv = inv_norm_from_sumsq(group_sum(s));
+      if (cinv && lane == 0) cinv[e] = inv;   // (KC == 1)
     }
     for (int c = lane; c < nchp; c += 8) {
       float4 x = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -460,8 +461,9 @@ bool tc_supported(const kge_model_t* m, int64_t nc) {
 
 // Candidate operands from the model's own fp32 tables src[k] (row pitch m->dim): bf16 split (+ norm
 // columns, + the per-row norm bounds) and, when `scratch` is given, the fp32 copy the fp32 fallback sweep reads
-// (normalised for TransE, zero padded to dp) — all in one kernel.
-int tc_prepare_candidates(const RankCall& C, const float* const src[2], float* scratch, cudaStream_t st) {
+// (normalised for TransE, zero padded to dp), or (TransE) when `cinv` is given the rows' inverse norms — all in
+// one kernel.
+int tc_prepare_candidates(const RankCall& C, const float* const src[2], float* scratch, float* cinv, cudaStream_t st) {
   const kge_model_t* m = C.m;
   const int64_t nc = C.nc;
   const int KC = rank_kq(m->model), d = m->dim, dp = rank_dp(m), Kp = tc_kp(m), aug = tc_kind(m) != 0 ? 1 : 0;
@@ -472,7 +474,7 @@ int tc_prepare_candidates(const RankCall& C, const float* const src[2], float* s
                         : (nrm ? tc_prep_cand_kernel<1, true> : tc_prep_cand_kernel<1, false>);
   kernel<<<(unsigned)((nc + 31) / 32), 256, 0, st>>>(
       src[0], KC == 2 ? src[1] : src[0], (int64_t)d, nc, d, dp, KC, Kp, aug, C.at<__nv_bfloat16>(C.L.b[0]),
-      C.at<__nv_bfloat16>(C.L.b[1]), C.at<float>(C.L.cn), scratch, (scratch && KC == 2) ? scratch + (size_t)nc * dp : nullptr);
+      C.at<__nv_bfloat16>(C.L.b[1]), C.at<float>(C.L.cn), scratch, (scratch && KC == 2) ? scratch + (size_t)nc * dp : nullptr, cinv);
   KGE_CHECK_LAUNCH("tc_prep_cand_kernel");
   return KGE_OK;
 }

@@ -15,7 +15,7 @@ struct TcQueryArgs {
                               //   centre, a, b, e :  half(q,c) = a + b n_c + e n_c^2 ;
                               //   certainly better: D - centre > half;  certainly not: D - centre < -half
   int32_t* tc_counts;         // [Q] zeroed here
-  unsigned* ctrl;             // [4] zeroed here: pair-list length, overflow (+ 2 unused words)
+  unsigned* ctrl;             // [4] zeroed here: pair-list length, overflow, done counter (+ 1 unused)
   int Kp, kind;               // padded contraction length; 0 dot, 1 squared distance (sum domain), 2 squared distance - margin
   float sign, margin;
 };

@@ -16,14 +16,15 @@
 // compute loop is a per-lane base plus a compile-time immediate.  Query vectors are prepared
 // once per call (prep_query_kernel, which also yields the thresholds) into a compact
 // [Q][KQ][dp] buffer; candidates come straight from the model tables (or from a normalised /
-// even-part / padded scratch copy).  Two modes, chosen on the host from the shared-memory
-// budget: whole rows (query block resident for the whole CTA) and slabs of DS <= 256 columns for
-// wide models (d = 500, 1000), accumulators living across slabs.
+// even-part / padded scratch copy; raw TransE rows are normalised in shared memory).  Two modes,
+// chosen on the host from the shared-memory budget: whole rows (query block resident for the whole
+// CTA) and slabs of DS <= 256 columns for wide models (d = 500, 1000), accumulators living across slabs.
 //
 // Bound: fp32 pipe (2-8 instructions per element pair), not HBM: a candidate row is read from
 // L2 once per query BLOCK instead of once per query.
 #include "kge_models.cuh"
 #include "kge_rank.cuh"
+#include "kge_rank_resolve.cuh"
 #include "kge_rank_tc.cuh"
 #include "kge_tma.cuh"
 
@@ -47,21 +48,17 @@ struct TiledParams {
   const float* qvec;      // [Q][KQ][dp]
   const float* cand[2];   // KC candidate arrays, row pitch cand_pitch floats
   int64_t cand_pitch;
+  const float* cand_inv;  // TransE on the raw table: [nc] inverse row norms the staged rows are scaled by, or nullptr
   const float* thr;       // [Q]
   const float* qscale;    // [Q] (TransM theta[r]) or nullptr
   int64_t Q, nc;
   int dp, DS, nslabs;
   int tiles_per_cta, ntiles;
+  int splits, units;      // work unit u = (run of tiles u % splits, query block u / splits); units = splits x blocks
   int32_t* counts;
   int col, l1;
   int fin;      // DOT ops: 0 -> -sum ; 1 -> -sigmoid(sum) (HoLE) ; 2 -> -clamp(sum, +-20) (SimplE)
   float margin;
-  // tensor-core path (tc_ctrl != nullptr): this sweep is enqueued behind the two levels as the exact fallback.
-  // When the ambiguous-pair list did NOT overflow (tc_ctrl[0] <= tc_cap and tc_ctrl[1] == 0) it only commits the
-  // direction — counts[q*4+col], counts[q*4+col+1] += tc_counts[q] — and returns; else it ranks the direction.
-  const unsigned* tc_ctrl;
-  unsigned tc_cap;
-  const int32_t* tc_counts;
 };
 
 // ---- per-element pair operations (canonical arithmetic) ---------------------------------------
@@ -144,7 +141,7 @@ KGE_DEV void reduce_scatter(float (&v)[NV], int lane) {
 struct TiledMaps { CUtensorMap q, c0, c1; };
 
 template <int OP, bool L1>
-__device__ __forceinline__ void sweep_tiled_body(const TiledParams& P, const TiledMaps& TM) {
+__device__ __forceinline__ void sweep_tiled_body(const TiledParams& P, const TiledMaps& TM, int unit) {
   constexpr int KQ = OpTraits<OP>::KQ, KC = OpTraits<OP>::KC, TQ = OpTraits<OP>::TQ;
   constexpr int QBLK = kGQ * TQ;
   constexpr int NV = TQ * kTC;
@@ -165,22 +162,10 @@ __device__ __forceinline__ void sweep_tiled_body(const TiledParams& P, const Til
   const int warp = __shfl_sync(0xffffffffu, tid >> 5, 0);
   const int g = (tid >> 3) & 3;
   const int gc = warp % kGC, gq = (warp / kGC) * 4 + g;
-  const int64_t q0 = (int64_t)blockIdx.y * QBLK;
+  const int64_t q0 = (int64_t)(unit / P.splits) * QBLK;
   const int qrows = (int)min((int64_t)QBLK, P.Q - q0);
-  const int t0 = blockIdx.x * P.tiles_per_cta;
+  const int t0 = (unit % P.splits) * P.tiles_per_cta;
   const int ntile_local = min(P.tiles_per_cta, P.ntiles - t0);
-  if (P.tc_ctrl != nullptr) {
-    const unsigned listed = *reinterpret_cast<const volatile unsigned*>(P.tc_ctrl);
-    const bool overflow = listed > P.tc_cap || *reinterpret_cast<const volatile unsigned*>(P.tc_ctrl + 1) != 0u;
-    if (!overflow) {   // the usual case: commit the tensor-core levels' counts (one thread per query) and leave
-      const int64_t q = ((int64_t)blockIdx.y * gridDim.x + blockIdx.x) * blockDim.x + threadIdx.x;
-      if (q < P.Q) {
-        const int c = __ldg(P.tc_counts + q);
-        if (c) { atomicAdd(P.counts + q * 4 + P.col, c); atomicAdd(P.counts + q * 4 + P.col + 1, c); }
-      }
-      return;
-    }
-  }
   if (ntile_local <= 0) return;
   const int T = ntile_local * P.nslabs;
   const bool sum_domain = (OP == OP_TRANS_T || OP == OP_TRANS_H) && !L1 && P.qscale == nullptr;
@@ -257,6 +242,21 @@ __device__ __forceinline__ void sweep_tiled_body(const TiledParams& P, const Til
         for (int i = 0; i < NV; ++i) acc[nt][i] = 0.f;
     }
     mbar_wait(&bars[stage], (uint32_t)((it >> 1) & 1));
+    if constexpr (OP == OP_TRANS_T || OP == OP_TRANS_H) {
+      if (P.cand_inv) {
+        // raw TransE rows: normalise the staged candidate tile once, with prep_cand_kernel's fmul(x, inv) (same
+        // bits as the scratch copy; columns past the row are zeros either way, rows past nc are left alone)
+        float* ct = reinterpret_cast<float*>(cbase + (size_t)stage * c_stage_bytes);
+        const int64_t r0 = (int64_t)tile * kCBLK;
+        const int nel = ((min(DS, P.dp - slab * DS) + 31) >> 5) * kCBLK * 32;   // [octet][row][32 floats]
+        for (int i = tid; i < nel; i += kTThreads) {
+          const int64_t row = r0 + ((i >> 5) % kCBLK);
+          if (row < P.nc) ct[i] = fmul(ct[i], __ldg(P.cand_inv + row));
+        }
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // before the stage's next TMA refill
+        __syncthreads();
+      }
+    }
     const int nch = min(DS, P.dp - slab * DS) >> 2;
     // lane's chunk c = 8*octet + lane of row r sits at  octet*OctBytes + r*128 + lane*16
     const unsigned char* qs = qbase + (size_t)(P.nslabs > 1 ? stage : 0) * q_stage_bytes + (gq * TQ * KQ) * 128 + lane * 16;
@@ -359,12 +359,55 @@ __device__ __forceinline__ void sweep_tiled_body(const TiledParams& P, const Til
 template <int OP, bool L1>
 __global__ void __launch_bounds__(kTThreads)
 sweep_tiled_kernel(const __grid_constant__ TiledParams P, const __grid_constant__ TiledMaps TM) {
-  sweep_tiled_body<OP, L1>(P, TM);
+  sweep_tiled_body<OP, L1>(P, TM, blockIdx.x);
 }
 template <int OP, bool L1>
 __global__ void __launch_bounds__(kTThreads, 2)
 sweep_tiled_kernel_2cta(const __grid_constant__ TiledParams P, const __grid_constant__ TiledMaps TM) {
-  sweep_tiled_body<OP, L1>(P, TM);
+  sweep_tiled_body<OP, L1>(P, TM, blockIdx.x);
+}
+
+// The tensor-core path's one launch per direction after the sweep.  The sweep has finished, so the pair list's
+// length and overflow flag are final:
+//   no overflow: resolve the band pairs (into tc_counts) and the filter entries; the last CTA to finish (fenced
+//                done counter ctrl[2], reset for the next call or graph replay) then commits the direction,
+//                counts[q][col], counts[q][col + 1] += tc_counts[q];
+//   overflow (degenerate tables): the fp32 tiled sweep of the direction, one work unit per CTA, then the filter
+//                corrections.
+// The fallback is a call of its own: inlined, its register pressure would spill into the resolve loop that
+// every call runs.
+template <int OP>
+__device__ __noinline__ void tiled_fallback(const TiledParams& P, const TiledMaps& TM, int unit) {
+  sweep_tiled_body<OP, false>(P, TM, unit);
+}
+
+// (2 CTAs per SM, as the resolve kernel of the gather and fp32 paths and the tiled sweep run: 128 registers)
+template <int MODEL, int VEC, int GROUPING, int OP>
+__global__ void __launch_bounds__(kTThreads, 2)
+tc_resolve_commit_kernel(const __grid_constant__ ModelParams MP, const __grid_constant__ ResolveArgs A,
+                         const __grid_constant__ TiledParams TP, const __grid_constant__ TiledMaps TM) {
+  extern __shared__ float4 smem_f4[];
+  float* scratch = reinterpret_cast<float*>(smem_f4) + (size_t)(threadIdx.x >> 3) * A.scratch_floats;
+  const unsigned listed = *reinterpret_cast<const volatile unsigned*>(A.ctrl);
+  const bool overflow = listed > A.cap || *reinterpret_cast<const volatile unsigned*>(A.ctrl + 1) != 0u;
+  if (overflow) {
+    if ((int)blockIdx.x < TP.units) tiled_fallback<OP>(TP, TM, blockIdx.x);
+    __syncthreads();   // the sweep's shared memory becomes the group scratch
+    resolve_items<MODEL, VEC, GROUPING>(MP, A, 0, scratch);
+    return;
+  }
+  resolve_items<MODEL, VEC, GROUPING>(MP, A, (int64_t)listed, scratch);
+  __threadfence();     // every thread's tc_counts updates, then the whole CTA, before its arrival on the done counter
+  __syncthreads();
+  unsigned prev = 0u;
+  if (threadIdx.x == 0) prev = atomicAdd(A.ctrl + 2, 1u);
+  if (!__syncthreads_or(threadIdx.x == 0 && prev == gridDim.x - 1)) return;
+  __threadfence();
+  for (int64_t q = threadIdx.x; q < A.Q; q += blockDim.x) {
+    const int c = __ldcg(A.tc_counts + q);
+    if (c) { atomicAdd(A.counts + q * 4 + A.col, c); atomicAdd(A.counts + q * 4 + A.col + 1, c); }
+  }
+  if (threadIdx.x == 0) A.ctrl[2] = 0u;
 }
 
 // ---- preparation kernels -------------------------------------------------------------------------
@@ -378,7 +421,7 @@ prep_query_kernel(ModelParams P, const int64_t* __restrict__ qh, const int64_t* 
   float* scratch = reinterpret_cast<float*>(smem_f4) + (size_t)(threadIdx.x >> 3) * scratch_floats;
   const int lane = threadIdx.x & 7;
   const int64_t q = (int64_t)blockIdx.x * 32 + (threadIdx.x >> 3);
-  if (TC.A0 && blockIdx.x == 0 && threadIdx.x < 4) TC.ctrl[threadIdx.x] = 0u;   // pair-list length, overflow (+ 2 unused words)
+  if (TC.A0 && blockIdx.x == 0 && threadIdx.x < 4) TC.ctrl[threadIdx.x] = 0u;   // pair-list length, overflow, done counter (+ 1 unused)
   if (q >= Q) return;
   const int d = P.d, nch = (d + 3) >> 2, nchp = dp >> 2;
   TripleRows R;
@@ -570,12 +613,21 @@ static int fill_cand_scratch(const RankCall& C, const float* const src[2], cudaS
   return KGE_OK;
 }
 
+// TransE on the tensor-core path: when TMA can read the table itself (rows of whole 16-byte chunks, 16-byte
+// aligned), the fp32 fallback stages the raw rows and normalises them in shared memory with the inverse norms
+// tc_prep_cand_kernel writes, instead of reading a normalised scratch copy that the usual call never needs
+static bool tc_raw_transe(const RankCall& C) {
+  return C.use_tc && C.m->model == KGE_TRANSE && C.m->dim % 4 == 0 && ((uintptr_t)C.m->tables[0] & 15) == 0;
+}
+
 int prepare_candidates(const RankCall& C, cudaStream_t st) {
   if (C.m->model == KGE_CP || is_simple(C.m->model)) return KGE_OK;  // per direction: prepare_queries / tiled_sweep
   const float* src[2];
   const bool scratch = cand_sources(C.m, 0, src);
-  if (C.use_tc)   // one kernel: bf16 split for the tensor cores + (if the fp32 sweep needs one) its scratch copy
-    return tc_prepare_candidates(C, src, scratch ? C.at<float>(C.L.cand) : nullptr, st);
+  if (C.use_tc) {  // one kernel: bf16 split for the tensor cores + what the fp32 fallback needs, if anything
+    if (tc_raw_transe(C)) return tc_prepare_candidates(C, src, nullptr, C.at<float>(C.L.cinv), st);
+    return tc_prepare_candidates(C, src, scratch ? C.at<float>(C.L.cand) : nullptr, nullptr, st);
+  }
   if (scratch) return fill_cand_scratch(C, src, st);
   return KGE_OK;
 }
@@ -596,7 +648,7 @@ int prepare_queries(const RankCall& C, int dir, cudaStream_t st) {
   if (m->model == KGE_CP && C.use_tc) {
     const float* src[2] = {nullptr, nullptr};
     const bool scratch = cand_sources(m, dir, src);
-    const int rc = tc_prepare_candidates(C, src, scratch ? C.at<float>(C.L.cand) : nullptr, st);
+    const int rc = tc_prepare_candidates(C, src, scratch ? C.at<float>(C.L.cand) : nullptr, nullptr, st);
     if (rc) return rc;
   }
   // query vectors and thresholds from the query-side tables
@@ -654,54 +706,31 @@ int make_tensor_map(CUtensorMap* tm, CUtensorMapDataType dtype, const void* base
   return KGE_OK;
 }
 
-template <int OP, bool L1>
-static int launch_sweep(const TiledParams& P, size_t smem, dim3 grid, SweepProfile* prof, cudaStream_t st) {
-  constexpr int KQ = OpTraits<OP>::KQ, KC = OpTraits<OP>::KC, QBLK = kGQ * OpTraits<OP>::TQ;
-  TiledMaps TM;
-  // fp32 matrices; one box = one octet: 32 columns x all rows of the tile (columns >= dp / rows >= extent read as zeros)
-  auto map = [&](CUtensorMap* tm, const float* base, uint64_t rows, uint64_t pitch, uint32_t box_rows) {
-    return make_tensor_map(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rows, (uint64_t)P.dp, pitch * sizeof(float), 32u,
-                           box_rows, CU_TENSOR_MAP_SWIZZLE_NONE);
-  };
-  int rc = map(&TM.q, P.qvec, (uint64_t)P.Q * KQ, (uint64_t)P.dp, (uint32_t)(QBLK * KQ));
-  if (rc) return rc;
-  rc = map(&TM.c0, P.cand[0], (uint64_t)P.nc, (uint64_t)P.cand_pitch, (uint32_t)kCBLK);
-  if (rc) return rc;
-  TM.c1 = TM.c0;
-  if (KC == 2) {
-    rc = map(&TM.c1, P.cand[1], (uint64_t)P.nc, (uint64_t)P.cand_pitch, (uint32_t)kCBLK);
-    if (rc) return rc;
-  }
-  const auto kernel = [] {
-    if constexpr (OP == OP_DOT2) return sweep_tiled_kernel_2cta<OP, L1>;
-    else return sweep_tiled_kernel<OP, L1>;
-  }();
-  rc = smem_optin(kernel, smem);
-  if (rc) return rc;
-  if (prof) KGE_CUDA_OK(cudaEventRecord(prof->beg, st));
-  kernel<<<grid, kTThreads, smem, st>>>(P, TM);
-  KGE_CHECK_LAUNCH("sweep_tiled_kernel");
-  if (prof) { KGE_CUDA_OK(cudaEventRecord(prof->end, st)); prof->valid = true; }
-  return KGE_OK;
-}
+// One direction's fp32 tiled sweep: parameters, tensor maps and launch shape (a 1-D grid of P.units CTAs).
+struct TiledPlan { TiledParams P; TiledMaps TM; size_t smem; int op; };
 
-int tiled_sweep(const RankCall& C, int dir, cudaStream_t st) {
+static int tiled_plan(const RankCall& C, int dir, cudaStream_t st, TiledPlan& T) {
   const kge_model_t* m = C.m;
   const int model = m->model, dp = rank_dp(m), KQ = rank_kq(model), KC = KQ;
   const int64_t Q = C.Q, nc = C.nc;
-  const int op = (model == KGE_TRANSE || model == KGE_TRANSM) ? (dir == 0 ? OP_TRANS_T : OP_TRANS_H)
-               : (model == KGE_DISTMULT || model == KGE_CP || model == KGE_HOLE || model == KGE_RESCAL) ? OP_DOT1
-               : (model == KGE_COMPLEX || is_simple(model)) ? OP_DOT2 : OP_ROT;
+  T.op = (model == KGE_TRANSE || model == KGE_TRANSM) ? (dir == 0 ? OP_TRANS_T : OP_TRANS_H)
+       : (model == KGE_DISTMULT || model == KGE_CP || model == KGE_HOLE || model == KGE_RESCAL) ? OP_DOT1
+       : (model == KGE_COMPLEX || is_simple(model)) ? OP_DOT2 : OP_ROT;
   const int TQ = 4;
   const int QBLK = kGQ * TQ;
+  TiledParams& P = T.P;
 
   // candidate arrays: the model's tables, or the scratch copy (made by prepare_candidates, or filled here
   // when the tables differ per direction)
-  TiledParams P;
+  P.cand_inv = nullptr;
   {
     const float* src[2] = {nullptr, nullptr};
     float* cscratch = C.at<float>(C.L.cand);
-    if (cand_sources(m, dir, src)) {
+    const bool scratch = cand_sources(m, dir, src);
+    if (tc_raw_transe(C)) {
+      P.cand[0] = src[0]; P.cand[1] = nullptr; P.cand_pitch = m->dim;
+      P.cand_inv = C.at<float>(C.L.cinv);
+    } else if (scratch) {
       for (int k = 0; k < KC; ++k) P.cand[k] = cscratch + (size_t)k * (size_t)nc * dp;
       if (KC == 1) P.cand[1] = nullptr;
       P.cand_pitch = dp;
@@ -730,36 +759,104 @@ int tiled_sweep(const RankCall& C, int dir, cudaStream_t st) {
     while (DS + 32 <= dp32 && DS + 32 <= 256 && bytes_for(DS + 32, 2) <= budget) DS += 32;
     nslabs = (dp + DS - 1) / DS;
   }
-  const size_t smem = bytes_for(DS, nslabs > 1 ? 2 : 1);
-  P.tc_ctrl = C.use_tc ? C.at<unsigned>(C.L.ctrl[dir]) : nullptr;
-  P.tc_cap = C.use_tc ? tc_list_capacity(Q) : 0;
-  P.tc_counts = C.use_tc ? C.at<int32_t>(C.L.tc_counts[dir]) : nullptr;
+  T.smem = bytes_for(DS, nslabs > 1 ? 2 : 1);
   P.qvec = C.at<float>(C.L.qvec[dir]); P.thr = C.thr(dir);
   P.qscale = (model == KGE_TRANSM) ? C.at<float>(C.L.qscale[dir]) : nullptr;
   P.Q = Q; P.nc = nc; P.dp = dp; P.DS = DS; P.nslabs = nslabs;
   P.ntiles = (int)((nc + kCBLK - 1) / kCBLK);
   const int qblocks = (int)((Q + QBLK - 1) / QBLK);
-  const int ctas_per_sm = (smem + 1024) * 2 <= 228 * 1024 ? 2 : 1;
+  const int ctas_per_sm = (T.smem + 1024) * 2 <= 228 * 1024 ? 2 : 1;
   int splits = (sm_count() * ctas_per_sm + qblocks - 1) / qblocks;
   if (splits < 1) splits = 1;
   if (splits > P.ntiles) splits = P.ntiles;
   P.tiles_per_cta = (P.ntiles + splits - 1) / splits;
   splits = (P.ntiles + P.tiles_per_cta - 1) / P.tiles_per_cta;
+  P.splits = splits; P.units = splits * qblocks;
   P.counts = C.counts; P.col = 2 * dir; P.l1 = m->l1_flag; P.margin = m->margin;
   P.fin = (model == KGE_HOLE) ? 1 : (is_simple(model) ? 2 : 0);
 
-  // with the tensor-core level the profiled kernel is tc_sweep_kernel
-  SweepProfile* prof = (sweep_profile(dir)->armed && !C.use_tc) ? sweep_profile(dir) : nullptr;
-  const dim3 grid((unsigned)splits, (unsigned)qblocks);
-  switch (op) {
-    case OP_TRANS_T: return m->l1_flag ? launch_sweep<OP_TRANS_T, true>(P, smem, grid, prof, st)
-                                       : launch_sweep<OP_TRANS_T, false>(P, smem, grid, prof, st);
-    case OP_TRANS_H: return m->l1_flag ? launch_sweep<OP_TRANS_H, true>(P, smem, grid, prof, st)
-                                       : launch_sweep<OP_TRANS_H, false>(P, smem, grid, prof, st);
-    case OP_DOT1: return launch_sweep<OP_DOT1, false>(P, smem, grid, prof, st);
-    case OP_DOT2: return launch_sweep<OP_DOT2, false>(P, smem, grid, prof, st);
-    default: return launch_sweep<OP_ROT, false>(P, smem, grid, prof, st);
+  // fp32 matrices; one box = one octet: 32 columns x all rows of the tile (columns >= dp / rows >= extent read as zeros)
+  auto map = [&](CUtensorMap* tm, const float* base, uint64_t rows, uint64_t pitch, uint32_t box_rows) {
+    return make_tensor_map(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, base, rows, (uint64_t)P.dp, pitch * sizeof(float), 32u,
+                           box_rows, CU_TENSOR_MAP_SWIZZLE_NONE);
+  };
+  int rc = map(&T.TM.q, P.qvec, (uint64_t)P.Q * KQ, (uint64_t)P.dp, (uint32_t)(QBLK * KQ));
+  if (rc) return rc;
+  rc = map(&T.TM.c0, P.cand[0], (uint64_t)P.nc, (uint64_t)P.cand_pitch, (uint32_t)kCBLK);
+  if (rc) return rc;
+  T.TM.c1 = T.TM.c0;
+  if (KC == 2) {
+    rc = map(&T.TM.c1, P.cand[1], (uint64_t)P.nc, (uint64_t)P.cand_pitch, (uint32_t)kCBLK);
+    if (rc) return rc;
   }
+  return KGE_OK;
+}
+
+template <int OP, bool L1>
+static int launch_sweep(const TiledPlan& T, SweepProfile* prof, cudaStream_t st) {
+  const auto kernel = [] {
+    if constexpr (OP == OP_DOT2) return sweep_tiled_kernel_2cta<OP, L1>;
+    else return sweep_tiled_kernel<OP, L1>;
+  }();
+  const int rc = smem_optin(kernel, T.smem);
+  if (rc) return rc;
+  if (prof) KGE_CUDA_OK(cudaEventRecord(prof->beg, st));
+  kernel<<<(unsigned)T.P.units, kTThreads, T.smem, st>>>(T.P, T.TM);
+  KGE_CHECK_LAUNCH("sweep_tiled_kernel");
+  if (prof) { KGE_CUDA_OK(cudaEventRecord(prof->end, st)); prof->valid = true; }
+  return KGE_OK;
+}
+
+int tiled_sweep(const RankCall& C, int dir, cudaStream_t st) {
+  TiledPlan T;
+  const int rc = tiled_plan(C, dir, st, T);
+  if (rc) return rc;
+  SweepProfile* prof = sweep_profile(dir)->armed ? sweep_profile(dir) : nullptr;
+  const bool l1 = C.m->l1_flag != 0;
+  switch (T.op) {
+    case OP_TRANS_T: return l1 ? launch_sweep<OP_TRANS_T, true>(T, prof, st) : launch_sweep<OP_TRANS_T, false>(T, prof, st);
+    case OP_TRANS_H: return l1 ? launch_sweep<OP_TRANS_H, true>(T, prof, st) : launch_sweep<OP_TRANS_H, false>(T, prof, st);
+    case OP_DOT1: return launch_sweep<OP_DOT1, false>(T, prof, st);
+    case OP_DOT2: return launch_sweep<OP_DOT2, false>(T, prof, st);
+    default: return launch_sweep<OP_ROT, false>(T, prof, st);
+  }
+}
+
+int tc_resolve_commit(const RankCall& C, int dir, cudaStream_t st) {
+  TiledPlan T;
+  int rc = tiled_plan(C, dir, st, T);
+  if (rc) return rc;
+  const GroupArgs G = group_args(C);
+  decltype(&tc_resolve_commit_kernel<KGE_TRANSE, 4, KGE_GROUP_TAIL, OP_TRANS_T>) kernel;
+#define PICK_OP(M, V, OP) kernel = dir == 0 ? tc_resolve_commit_kernel<M, V, KGE_GROUP_TAIL, OP> \
+                                            : tc_resolve_commit_kernel<M, V, KGE_GROUP_HEAD, OP>
+#define PICK_TRANSE(M, V) kernel = dir == 0 ? tc_resolve_commit_kernel<M, V, KGE_GROUP_TAIL, OP_TRANS_T> \
+                                            : tc_resolve_commit_kernel<M, V, KGE_GROUP_HEAD, OP_TRANS_H>
+#define PICK_DOT1(M, V) PICK_OP(M, V, OP_DOT1)
+#define PICK_DOT2(M, V) PICK_OP(M, V, OP_DOT2)
+#define PICK_ROT(M, V) PICK_OP(M, V, OP_ROT)
+  switch (C.m->model) {   // the models tc_supported admits
+    case KGE_TRANSE: KGE_DISPATCH_VEC(KGE_TRANSE, G.vec, PICK_TRANSE); break;
+    case KGE_DISTMULT: KGE_DISPATCH_VEC(KGE_DISTMULT, G.vec, PICK_DOT1); break;
+    case KGE_CP: KGE_DISPATCH_VEC(KGE_CP, G.vec, PICK_DOT1); break;
+    case KGE_RESCAL: KGE_DISPATCH_VEC(KGE_RESCAL, G.vec, PICK_DOT1); break;
+    case KGE_COMPLEX: KGE_DISPATCH_VEC(KGE_COMPLEX, G.vec, PICK_DOT2); break;
+    case KGE_ROTATE: KGE_DISPATCH_VEC(KGE_ROTATE, G.vec, PICK_ROT); break;
+    default: set_error("tc_resolve_commit: model %d has no tensor-core path", (int)C.m->model); return KGE_ENOTSUP;
+  }
+#undef PICK_ROT
+#undef PICK_DOT2
+#undef PICK_DOT1
+#undef PICK_TRANSE
+#undef PICK_OP
+  const size_t smem = T.smem > G.smem ? T.smem : G.smem;
+  rc = smem_optin(kernel, smem);
+  if (rc) return rc;
+  // band pairs and filter entries grid-stride over two CTAs per SM; the fallback needs one CTA per work unit
+  const int grid = T.P.units > 2 * sm_count() ? T.P.units : 2 * sm_count();
+  kernel<<<(unsigned)grid, kTThreads, smem, st>>>(G.P, resolve_args(C, dir), T.P, T.TM);
+  KGE_CHECK_LAUNCH("tc_resolve_commit_kernel");
+  return KGE_OK;
 }
 
 }  // namespace kge
