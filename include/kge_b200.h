@@ -362,6 +362,43 @@ int kge_proj_rank(const float* x, const float* ent, const float* bias, int64_t Q
                   int32_t direction, int32_t* counts, void* workspace, int64_t workspace_bytes,
                   void* stream);
 
+/* ---- batched top-k link prediction --------------------------------------------------------------------
+ * The k most plausible candidates of Q queries at once, best first, with known positives optionally left out.
+ * Replaces the reference's per-query prediction route: Evaluator.test_tail_rank / test_head_rank /
+ * test_rel_rank (pykg2vec/utils/evaluator.py:249-287: one N-wide forward and a full topk per query, in
+ * DESCENDING forward score, i.e. worst first for every pairwise / pointwise model), Trainer.infer_tails /
+ * infer_heads / infer_rels (pykg2vec/utils/trainer.py:330-386) and predict_tail_rank / predict_head_rank of the
+ * projection models (pykg2vec/models/projection.py:119-125).  Those entry points keep their contract; these are
+ * the batched alternative.  Design: DESIGN.md §8, kernels: pykg2vec_b200/csrc/kge_topk.cuh.
+ *   out_ids[q*k + j] (int64), out_scores[q*k + j] (fp32), j = 0 best.
+ * Order: kernel models lowest score first (lower is more plausible, kge_score_fwd's convention); projection
+ * models highest sigmoid(x.E^T + b) first.  Equal scores: smaller id first; -0 == +0; NaN after every number.
+ * The result is the same on every run.  Scores are bit-identical to what the rank path compares: tails
+ * kge_rank_1vsall's TAIL sweep, heads its HEAD sweep, relations kge_score_fwd in TAIL grouping over (h, r', t),
+ * projection models kge_proj_tail_fwd.
+ * Filter: optional CSR over the queries (ptr[Q+1], idx[nnz], global candidate ids, the layout of kge_rank_1vsall;
+ * NULL / nnz 0: raw).  Listed candidates are removed entirely; duplicates are harmless, ids outside the candidate
+ * range are ignored.  When fewer than k candidates remain the list ends in id -1, score NaN.
+ * Limits: 1 <= k <= 256, Q >= 0 (Q = 0: nothing happens); KGE_EINVAL for anything else, a bad target or a NULL
+ * pointer the call needs, KGE_EWORKSPACE for a short workspace, all before any launch.  KGE_ENOTSUP when the
+ * candidate count is so large (> ~1.8 M) that the filter bitmap does not fit in shared memory.
+ * workspace >= kge_topk_workspace_bytes(Q, n_cand, k) bytes of device memory (0 for invalid arguments): one fp32
+ * score block of a chunk of queries — the launchers loop over chunks of max(1, min(65535, 64 MiB / (4 n_cand)))
+ * queries, so it is at most max(64 MiB, 4 n_cand) bytes whatever Q.  No host synchronisation, no allocation. */
+int64_t kge_topk_workspace_bytes(int64_t Q, int64_t n_cand, int32_t k);
+/* Kernel models.  target 0: tails of (qh, qr) over the num_ent entities; 1: heads of (qr, qt); 2: relations of
+ * (qh, qt) over the num_rel relations.  The array at the predicted position is ignored and may be NULL.
+ * Rescal normalises its rows in the reference's forward(): callers apply that first, as for kge_rank_1vsall. */
+int kge_topk_1vsall(const kge_model_t* m, int32_t target, const int64_t* qh, const int64_t* qr,
+                    const int64_t* qt, int64_t Q, int32_t k, const int64_t* filt_ptr, const int64_t* filt_idx,
+                    int64_t filt_nnz, int64_t* out_ids, float* out_scores, void* workspace,
+                    int64_t workspace_bytes, void* stream);
+/* Projection models: x [Q, width] is the trunk's output (the operand kge_proj_rank takes), ent [N, width],
+ * bias [N] or NULL; candidates are the N entities. */
+int kge_proj_topk(const float* x, const float* ent, const float* bias, int64_t Q, int64_t N, int32_t width,
+                  int32_t k, const int64_t* filt_ptr, const int64_t* filt_idx, int64_t filt_nnz, int64_t* out_ids,
+                  float* out_scores, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- ConvE trunk, inference mode ----------------------------------------------------------
  * ConvE.forward + inner_forward up to the x.E^T product (pykg2vec/models/projection.py:104-112,
  * :86-99) with self.training == False: x[q,:] = relu(fc(flatten(relu(bn1(conv2d_1(bn0(

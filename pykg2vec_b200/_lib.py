@@ -43,6 +43,7 @@ EXPORTS = [
     "kge_interacte_train_workspace_bytes", "kge_interacte_train_fwd", "kge_interacte_train_bwd",
     "kge_acre_train_workspace_bytes", "kge_acre_train_fwd", "kge_acre_train_bwd",
     "kge_project_entities", "kge_normalize_rows_to",
+    "kge_topk_workspace_bytes", "kge_topk_1vsall", "kge_proj_topk",
 ]
 
 
@@ -92,6 +93,7 @@ def lib():
     L.kge_hyper_train_workspace_bytes.restype = ctypes.c_int64
     L.kge_interacte_train_workspace_bytes.restype = ctypes.c_int64
     L.kge_acre_train_workspace_bytes.restype = ctypes.c_int64
+    L.kge_topk_workspace_bytes.restype = ctypes.c_int64
     if L.kge_abi_version() != ABI_VERSION:
         raise KgeError("libkge_b200.so ABI %d != binding ABI %d" % (L.kge_abi_version(), ABI_VERSION))
     missing = [name for name in EXPORTS if not hasattr(L, name)]
@@ -513,6 +515,70 @@ def proj_rank(x, ent, bias, tgt, filt=None, direction=0, counts=None, workspace=
                               _ptr(counts), _ptr(workspace), ctypes.c_int64(workspace.numel()), _stream()),
           "kge_proj_rank")
     return counts
+
+
+# ---- batched top-k link prediction (include/kge_b200.h: kge_topk_*, kge_proj_topk) ---------------------
+TOPK_TAIL, TOPK_HEAD, TOPK_REL = 0, 1, 2
+TOPK_MAX_K = 256
+
+
+def topk_workspace_bytes(Q, n_cand, k):
+    return int(lib().kge_topk_workspace_bytes(ctypes.c_int64(Q), ctypes.c_int64(n_cand), ctypes.c_int32(k)))
+
+
+def _topk_out(Q, k, n_cand, device, workspace):
+    if not 1 <= int(k) <= TOPK_MAX_K:
+        raise KgeError("k must be in [1, %d], got %r" % (TOPK_MAX_K, k))
+    ids = torch.empty((Q, k), dtype=torch.int64, device=device)
+    scores = torch.empty((Q, k), dtype=torch.float32, device=device)
+    nbytes = topk_workspace_bytes(Q, n_cand, k)
+    if workspace is None or workspace.numel() < nbytes:
+        workspace = torch.empty(max(nbytes, 16), dtype=torch.uint8, device=device)
+    return ids, scores, workspace
+
+
+def _filt_args(filt):
+    fp, fi = filt if filt is not None else (None, None)
+    if fp is not None:
+        fp, fi = _dev_i64(fp, "filt ptr"), _dev_i64(fi, "filt idx")
+    return _ptr(fp), _ptr(fi), ctypes.c_int64(fi.numel() if fi is not None else 0)
+
+
+def topk_1vsall(desc, target, qh, qr, qt, k, filt=None, workspace=None):
+    """The k best candidates of each query, best (lowest score) first -> (ids [Q,k] int64, scores [Q,k] fp32) on the
+    device.  target TOPK_TAIL: tails of (qh, qr); TOPK_HEAD: heads of (qr, qt); TOPK_REL: relations of (qh, qt); the
+    ids at the predicted position may be None.  filt = (ptr[Q+1], idx[nnz]) CSR of candidates to leave out, or None.
+    Fewer than k candidates left: id -1, score NaN."""
+    if target not in (TOPK_TAIL, TOPK_HEAD, TOPK_REL):
+        raise KgeError("target must be 0 (tail), 1 (head) or 2 (relation)")
+    predicted = {TOPK_TAIL: 2, TOPK_HEAD: 0, TOPK_REL: 1}[target]   # the id array the call ignores
+    q = [None if (a is None or i == predicted) else _dev_i64(a, name)
+         for i, (a, name) in enumerate(((qh, "qh"), (qr, "qr"), (qt, "qt")))]
+    ref = next(a for a in q if a is not None)
+    Q = ref.numel()
+    n_cand = desc.num_rel if target == TOPK_REL else desc.num_ent
+    ids, scores, workspace = _topk_out(Q, k, n_cand, ref.device, workspace)
+    m = desc.c_struct()
+    check(lib().kge_topk_1vsall(ctypes.byref(m), ctypes.c_int32(target), _ptr(q[0]), _ptr(q[1]), _ptr(q[2]),
+                                ctypes.c_int64(Q), ctypes.c_int32(k), *_filt_args(filt), _ptr(ids), _ptr(scores),
+                                _ptr(workspace), ctypes.c_int64(workspace.numel()), _stream()), "kge_topk_1vsall")
+    return ids, scores
+
+
+def proj_topk(x, ent, bias, k, filt=None, workspace=None):
+    """The k entities with the highest sigmoid(x . ent^T + bias) per row of x, best first -> (ids [Q,k] int64,
+    scores [Q,k] fp32) on the device; filt as for topk_1vsall."""
+    x, ent = _dev_f32(x, "x"), _dev_f32(ent, "ent")
+    if x.dim() != 2 or ent.dim() != 2 or x.shape[1] != ent.shape[1]:
+        raise KgeError("x must be [Q,k] and ent [N,k]")
+    Q, width = x.shape
+    N = ent.shape[0]
+    bias = _bias_row(bias, N)
+    ids, scores, workspace = _topk_out(Q, k, N, x.device, workspace)
+    check(lib().kge_proj_topk(_ptr(x), _ptr(ent), _ptr(bias), ctypes.c_int64(Q), ctypes.c_int64(N),
+                              ctypes.c_int32(width), ctypes.c_int32(k), *_filt_args(filt), _ptr(ids), _ptr(scores),
+                              _ptr(workspace), ctypes.c_int64(workspace.numel()), _stream()), "kge_proj_topk")
+    return ids, scores
 
 
 class KgeConve(ctypes.Structure):

@@ -364,6 +364,100 @@ class Evaluator:
             self.last_d2h_bytes += q * 16
         return out
 
+    # ---- batched top-k prediction ------------------------------------------------------------------
+    def predict_tails(self, hs, rs, k=10, filtered=False):
+        """The k most plausible tails of every (h, r) -> numpy (ids [Q,k] int64, scores [Q,k] float32), best first
+        (lowest score for the pairwise / pointwise models, highest prediction for the projection models; equal
+        scores by smaller id).  filtered=True leaves out the known tails of (h, r) from every split (hr_t).  Fewer
+        than k candidates left: id -1, score NaN.  The batched counterpart of test_tail_rank, which keeps the
+        reference's one-query, descending-score contract."""
+        hs, rs = self._topk_ids(hs, self.config.tot_entity, "h"), self._topk_ids(rs, self.config.tot_relation, "r")
+        if len(hs) != len(rs):
+            raise ValueError("hs and rs must have the same length")
+        filt = build_filter_csr(list(zip(hs.tolist(), rs.tolist())), self.metric_calculator.hr_t) if filtered else None
+        return self._predict(_lib.TOPK_TAIL, (hs, rs, None), k, filt)
+
+    def predict_heads(self, rs, ts, k=10, filtered=False):
+        """The k most plausible heads of every (r, t); see predict_tails (filter: tr_h)."""
+        rs, ts = self._topk_ids(rs, self.config.tot_relation, "r"), self._topk_ids(ts, self.config.tot_entity, "t")
+        if len(rs) != len(ts):
+            raise ValueError("rs and ts must have the same length")
+        filt = build_filter_csr(list(zip(ts.tolist(), rs.tolist())), self.metric_calculator.tr_h) if filtered else None
+        return self._predict(_lib.TOPK_HEAD, (None, rs, ts), k, filt)
+
+    def predict_rels(self, hs, ts, k=10):
+        """The k most plausible relations of every (h, t); see predict_tails.  Projection models score entities
+        only and raise KgeNotSupported, as the reference's infer_rels refuses them (trainer.py:367-369)."""
+        if hasattr(self.model, "proj_query"):
+            raise _lib.KgeNotSupported("predict_rels: projection models predict entities only")
+        hs, ts = self._topk_ids(hs, self.config.tot_entity, "h"), self._topk_ids(ts, self.config.tot_entity, "t")
+        if len(hs) != len(ts):
+            raise ValueError("hs and ts must have the same length")
+        return self._predict(_lib.TOPK_REL, (hs, None, ts), k, None)
+
+    @staticmethod
+    def _topk_ids(a, bound, name):
+        a = np.ascontiguousarray(np.asarray(a).reshape(-1), dtype=np.int64)
+        if a.size and (a.min() < 0 or a.max() >= bound):
+            raise ValueError("%s ids must lie in [0, %d)" % (name, bound))
+        return a
+
+    def _predict(self, target, qs, k, filt):
+        """Per batch of <= QUERY_BATCH queries: the query ids and filter rows go up in one pinned copy, the top-k
+        kernels run, ids and scores come back."""
+        if not 1 <= int(k) <= _lib.TOPK_MAX_K:
+            raise ValueError("k must be in [1, %d]" % _lib.TOPK_MAX_K)
+        k = int(k)
+        dev = self._dev()
+        Q = len(next(a for a in qs if a is not None))
+        ids = np.empty((Q, k), dtype=np.int64)
+        scores = np.empty((Q, k), dtype=np.float32)
+        proj = hasattr(self.model, "proj_query")
+        kw = {}
+        if proj:
+            ent, bias = self.model.proj_tail_tables()
+            ent = ent.detach()
+            bias = bias.detach() if bias is not None else None
+            make_cores = getattr(self.model, "proj_query_cores", None)   # TuckER: built per call, never kept
+            cores = make_cores(torch.from_numpy(np.unique(qs[1])).to(dev)) if make_cores is not None and Q else None
+            if cores is not None:
+                kw["cores"] = cores
+        else:
+            if not getattr(self.model, "kge_dense_params", False) and hasattr(self.model, "kge_pre_score"):
+                self.model.kge_pre_score()   # Rescal: tables row-normalised in place, as the reference's forward() does
+            desc = self.model.kge_desc()     # rebuilt per call: ConvKB derives its tables from the parameters
+        with torch.no_grad():
+            for lo in range(0, Q, self.QUERY_BATCH):
+                hi = min(Q, lo + self.QUERY_BATCH)
+                parts = [a[lo:hi] for a in qs if a is not None]
+                if filt is not None:
+                    ptr, idx = filt
+                    parts += [ptr[lo:hi + 1] - ptr[lo], idx[ptr[lo]:ptr[hi]]]
+                words = sum(len(a) for a in parts)
+                stage = getattr(self, "_topk_stage", None)
+                if stage is None or stage.numel() < words:   # pinned staging buffer, grown geometrically
+                    stage = self._topk_stage = torch.empty(max(words, 2 * (stage.numel() if stage is not None else 0)),
+                                                           dtype=torch.int64).pin_memory()
+                buf, o, views = stage.numpy(), 0, []
+                for a in parts:
+                    buf[o:o + len(a)] = a
+                    views.append((o, o + len(a)))
+                    o += len(a)
+                d_in = stage[:words].to(dev, non_blocking=True)
+                v = [d_in[a:b] for a, b in views]
+                f = (v[-2], v[-1]) if filt is not None and len(parts[-1]) else None
+                q = iter(v)
+                dq = [None if a is None else next(q) for a in qs]
+                if proj:
+                    e, direction = (dq[0], "tail") if target == _lib.TOPK_TAIL else (dq[2], "head")
+                    x = self.model.proj_query(e, dq[1], direction=direction, **kw).contiguous()
+                    out = _lib.proj_topk(x, ent, bias, k, f)
+                else:
+                    out = _lib.topk_1vsall(desc, target, dq[0], dq[1], dq[2], k, f)
+                ids[lo:hi] = out[0].cpu().numpy()
+                scores[lo:hi] = out[1].cpu().numpy()
+        return ids, scores
+
     @staticmethod
     def _bucket(n):
         cap = 256
