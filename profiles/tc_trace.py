@@ -38,9 +38,20 @@ spans = raw[192:].reshape(1024, 2)
 spans = spans[spans[:, 0] != 0]
 t0 = t[2, 63]
 out = {"directions": _lib.rank_last_sweep_directions(), "kernel_ms_untraced": times, "kernel_ms_traced": ms}
-# role 0: the TMA producer's stage waits; 1: consumer warpgroup start (warp 4); 2: epilogue begin / end per tile
-for r, name in enumerate(("producer", "consumer_start", "epilogue")):
+# role 0: the TMA producer's start, then one stamp per k-block issued (after its empty-barrier wait);
+# 1: consumer warpgroup start (warp 4), then one stamp per k-block after its full-barrier wait;
+# 2: epilogue begin / end per tile
+for r, name in enumerate(("producer", "consumer", "epilogue")):
     out[name] = [int(x - t0) for x in t[r, :62] if x != 0]
+prod, full, epi = out["producer"][1:], out["consumer"][1:], out["epilogue"]
+ntile = len(epi) // 2
+nkb = len(full) // ntile if ntile else 0
+# per tile: first k-block's operands in hand -> last MMA retired (compare with the tensor time of a tile)
+out["tile_mma_span_cycles"] = [epi[2 * i] - full[nkb * i] for i in range(ntile)] if nkb else []
+# per k-block: the producer's TMA issue -> the consumer past the full barrier (about one TMA round trip when
+# the consumers wait for operands, longer when the operands wait in the ring for the MMAs)
+out["ready_lag_cycles"] = [f - p for f, p in zip(full, prod)]
+out["starved_cycles"] = int(t[1, 63])   # warp 4's cycles inside full-barrier waits, summed
 if len(spans):
     s0 = spans[:, 0].min()
     out["ctas"] = int(len(spans))

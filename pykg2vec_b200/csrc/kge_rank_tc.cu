@@ -112,10 +112,13 @@ KGE_DEV void tc_wgmma(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t a
       : "memory");
 }
 
-// timeline stamps of CTA (0,0) (measurement aid; P.trace is null in normal operation)
+// timeline stamps of CTA (0,0) (measurement aid; P.trace is null in normal operation).  `slot` is evaluated
+// once: callers pass counters with side effects (ev++).
 #define TC_STAMP(role, slot)                                                                         \
   do {                                                                                               \
-    if (P.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (slot) < 64 && ((slot) < 62 || (slot) == 63)) P.trace[(role) * 64 + (slot)] = clock64(); \
+    const int tc_slot_ = (slot);                                                                     \
+    if (P.trace && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0 && (tc_slot_ < 62 || tc_slot_ == 63)) \
+      P.trace[(role) * 64 + tc_slot_] = clock64();                                                   \
   } while (0)
 
 // Pair-list slots are handed out per WARP in blocks (16 slots) reserved with one global atomic (a returning
@@ -154,10 +157,12 @@ KGE_DEV void tc_band_eval(const TcBand& Bq, float x, float n, float& u, float& h
 // Epilogue of one 64 x 128 accumulator tile held by a warpgroup: this thread's rows qa (= q of i = 0) and qa + 8,
 // columns 8j + 2(lane%4) + c of the tile (cbase + ...).  Counts the certainly-better candidates per row; warps in
 // which some pair lies inside its band list those pairs (a warp-level exclusive scan assigns the slots).
+// The band test runs once per pair: its in-band outcomes are kept as bits 4j + 2c + i of band[2] (j < 8 in band[0]),
+// and the listing walks the set bits — a handful per tile in a warp — instead of re-testing all 64 pairs.
 KGE_DEV void tc_epilogue(const float (&acc)[64], const float (&nl)[32], const TcBand (&Bq)[2], int64_t qa, int64_t cbase,
                          int nvalid, const TcParams& P, const TcDirView& V, TcListState& L, int lane, int (&cnt)[2]) {
   const int cl = 2 * (lane & 3);
-  int amb = 0;
+  unsigned band[2] = {0u, 0u};
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
 #pragma unroll
@@ -168,10 +173,11 @@ KGE_DEV void tc_epilogue(const float (&acc)[64], const float (&nl)[32], const Tc
         float u, h;
         tc_band_eval(Bq[i], acc[4 * j + 2 * i + c], nl[2 * j + c], u, h);
         cnt[i] += (ok && u > h) ? 1 : 0;
-        amb += (ok && u >= -h && !(u > h)) ? 1 : 0;
+        band[j >> 3] |= (ok && u >= -h && !(u > h)) ? 1u << ((4 * j + 2 * c + i) & 31) : 0u;
       }
     }
   }
+  const int amb = __popc(band[0]) + __popc(band[1]);
   if (__any_sync(0xffffffffu, amb != 0)) {
     int incl = amb;
 #pragma unroll
@@ -185,22 +191,13 @@ KGE_DEV void tc_epilogue(const float (&acc)[64], const float (&nl)[32], const Tc
       tc_list_reserve(L, P, V, lane, total > kTcListBlock ? total : kTcListBlock);
     }
     unsigned k = L.base + L.used + (unsigned)(incl - amb);
-    if (amb) {
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
-#pragma unroll
-        for (int c = 0; c < 2; ++c) {
-          const int col = 8 * j + cl + c;
-#pragma unroll
-          for (int i = 0; i < 2; ++i) {
-            float u, h;
-            tc_band_eval(Bq[i], acc[4 * j + 2 * i + c], nl[2 * j + c], u, h);
-            if (col < nvalid && u >= -h && !(u > h)) {
-              if (k < P.cap) V.list[k] = ((unsigned long long)(qa + 8 * i) << 32) | (unsigned long long)(cbase + col);
-              ++k;
-            }
-          }
-        }
+    for (int w = 0; w < 2; ++w) {
+      for (unsigned m = band[w]; m != 0u; m &= m - 1u) {   // ascending bits: the order of the pairs is (j, c, i)
+        const int b = 32 * w + __ffs(m) - 1;
+        const int i = b & 1, col = 8 * (b >> 2) + cl + ((b >> 1) & 1);
+        if (k < P.cap) V.list[k] = ((unsigned long long)(qa + 8 * i) << 32) | (unsigned long long)(cbase + col);
+        ++k;
       }
     }
     L.used += total;
@@ -320,8 +317,11 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
     int cnt[2] = {0, 0};
     TcListState L = {0u, 0u, 0u};
     tc_list_reserve(L, P, V, lane, kTcListBlock);   // the warp's first block: the atomic's round trip hides behind the first tile's MMAs
-    const bool stamper = warp == 4 && lane == 0;
-    int ev = 0;
+    // timeline of CTA (0,0,0), warp 4: role 1 = start, then one stamp after each full-barrier wait (slot 63: the
+    // cycles spent inside those waits, i.e. starved of operands); role 2 = epilogue begin / end per tile
+    const bool stamper = P.trace && warp == 4 && lane == 0;
+    int ev = 0, evf = 1;
+    long long starved = 0;
     if (stamper) TC_STAMP(1, ev++);
     int stage = 0; uint32_t phase = 0;
     float acc[64];
@@ -342,7 +342,9 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
         }
       int prev = -1;
       for (int kb = 0; kb < P.nkb; ++kb) {
+        const long long tw = stamper ? clock64() : 0;
         mbar_wait(&full[stage], phase);
+        if (stamper) { TC_STAMP(1, evf++); starved += clock64() - tw; }
         const uint32_t sb = st_base + (uint32_t)stage * st_bytes;
         const uint32_t a0 = (P.a_resident ? a_base + (uint32_t)kb * 2u * tb : sb + 2u * tb) + a_off;
         const uint64_t da0 = tc_smem_desc(a0), da1 = tc_smem_desc(a0 + tb);
@@ -369,6 +371,7 @@ tc_sweep_kernel(const __grid_constant__ TcParams P, const __grid_constant__ TcMa
       tc_epilogue(acc, nl, Bq, qa, cbase, nvalid, P, V, L, lane, cnt);
       if (stamper) TC_STAMP(2, ev++);
     }
+    if (stamper && blockIdx.x == 0 && blockIdx.y == 0 && blockIdx.z == 0) P.trace[64 + 63] = starved;
     tc_list_pad(L, P, V, lane);   // the unused slots of the warp's last block become holes
 #pragma unroll
     for (int i = 0; i < 2; ++i) {   // the four lanes of a row hold its 32 columns each
